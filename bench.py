@@ -44,7 +44,7 @@ MODEL_KEY, TABLE = "t2v-1.3B", "wan2.1_t2v_1.3b"
 
 def select_workload(name):
     """Default = BASELINE configs[1]. `wan14b` = configs[4]'s model and resolution (Wan2.1-T2V-14B, 1280x720x81f, E024K6R02):
-    not what the driver times, kept to show the 14B shapes run at full size (one GPU holds it: 28 GB of bf16 weights)."""
+    not the default workload, kept to show the 14B shapes run at full size (one GPU holds it: 28 GB of bf16 weights)."""
     global GRID, LATENT, PRESET, N_TOK, D, FFN, HEADS, LAYERS, ATTN_SELF_FLOPS, FWD_FLOPS, WORKLOAD, MODEL_KEY, TABLE
     if name == "wan14b":
         GRID, LATENT = (21, 45, 80), (16, 21, 90, 160)
@@ -62,11 +62,11 @@ def peaks():
         with open(p) as f:
             d = json.load(f)
         return dict(hbm_gbs=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src="fallback")
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=989.0, src="H100 SXM data sheet (dense bf16, 700 W), not measured")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -335,6 +335,12 @@ def run_ours(args, rank, world):
     live_tags = {"attn_self", "head", "head_hit_fused"}  # recorded live inside the timed region; the full attribution runs separately
     ms, launches, clocks, prof, x_final, per_fwd = timed(step_resident, args.steps, False if graphs else live_tags, args.warmup)
     assert torch.isfinite(x_final).all(), "non-finite latents after the timed steps"
+    if args.dump_outputs and rank == 0:
+        # the latent the last timed step returned (what a caller of cfg_denoise_step receives); the inputs are seeded, so two builds
+        # run with the same arguments can be compared output for output
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "latent.npy"), x_final.float().cpu().numpy())
     ms_e2e, _, _, _, _, _ = timed(step_e2e, args.steps, False, args.warmup)
     roofline_source = "CUDA events around every launch inside the timed region"
 
@@ -379,7 +385,7 @@ def run_ours(args, rank, world):
             traffic = json.load(f)["traffic_bytes_per_launch"]
     if "attn_self" in kern:
         ach = (ATTN_SELF_FLOPS / world) / (kern["attn_self"]["ms_avg"] * 1e-3) / 1e12  # per GPU: N/world query rows x N keys
-        roof = {"kernel": f"attn_long_kernel (self-attention, {N_TOK}x{N_TOK}x{HEADS} heads)", "bound": "tensor", "achieved": ach, "peak": pk["tf_sustained"],
+        roof = {"kernel": f"attn_kernel<128> (self-attention, {N_TOK}x{N_TOK}x{HEADS} heads)", "bound": "tensor", "achieved": ach, "peak": pk["tf_sustained"],
                 "unit": "TFLOP/s", "frac": ach / pk["tf_sustained"], "traffic": traffic, "peak_source": pk["src"] + " (sustained bf16)",
                 "share_of_step": (kern["attn_self"]["ms_total"] / ms) if not graphs else None, "flops_per_launch": ATTN_SELF_FLOPS / world,
                 "measured": roofline_source}
@@ -443,7 +449,7 @@ def run_ours(args, rank, world):
                        "parallelism": "single GPU" if world == 1 else f"token-axis shard over {world} GPUs ({N_TOK // world} tokens each), K|V rows exchanged per layer, replicated weights",
                        "cuda_graphs": bool(graphs),
                        "warmup_walks": f"steps {WARM_START_STEP}..{WARM_START_STEP + args.warmup - 1} of the schedule (misses and hits on both CFG slots), outside the timed region",
-                       "l2_policy": "per-forward working set (>= 1.3 GB of activations + 2.8 GB weights) exceeds the 126 MB L2; no explicit flush"},
+                       "l2_policy": "per-forward working set (>= 1.3 GB of activations + 2.8 GB weights) exceeds the 50 MB L2; no explicit flush"},
             "sec_per_video": sec_video,
             "sec_per_video_how": f"{n_miss_video} x t_miss + {n_hit_video} x t_hit + 50 x t_glue from the per-forward CUDA events of the timed region "
                                  f"(t_miss {t_miss and round(t_miss, 3)} ms, t_hit {t_hit and round(t_hit, 3)} ms, t_glue {round(t_glue, 3)} ms)",
@@ -598,7 +604,7 @@ def run_mmdit(args, rank, world):
     roof = None
     if "mmdit_attn" in kern:
         ach = attn_flops / (kern["mmdit_attn"]["ms_avg"] * 1e-3) / 1e12
-        roof = {"kernel": f"attn_long_kernel (joint attention, {n_img // world + n_txt}x{S}x{heads} heads per GPU)", "bound": "tensor", "achieved": ach, "peak": pk["tf_sustained"], "unit": "TFLOP/s",
+        roof = {"kernel": f"attn_kernel<128> (joint attention, {n_img // world + n_txt}x{S}x{heads} heads per GPU)", "bound": "tensor", "achieved": ach, "peak": pk["tf_sustained"], "unit": "TFLOP/s",
                 "frac": ach / pk["tf_sustained"], "traffic": None, "peak_source": pk["src"] + " (sustained bf16)", "share_of_step": kern["mmdit_attn"]["ms_total"] / ms,
                 "flops_per_launch": attn_flops, "measured": "CUDA events around every launch inside the timed region"}
     line = {"metric": "denoising_steps_per_sec", "value": steps / (ms * 1e-3), "unit": "steps/s", "n_gpus": world, "steps": steps, "warmup": args.warmup,
@@ -672,7 +678,7 @@ def bench_k1(dev, pk):
 def bench_hit_head(eng, algorithmic_bytes, pk):
     """The hit branch's kernel exactly as the path launches it (bf16 patch embedding + the slot's fp32 residual -> fp32 prediction,
     no step epilogue), 30 launches queued back to back on the engine's buffers of the last forward; every launch streams 302 MB
-    (> the 126 MB L2)."""
+    (> the 50 MB L2)."""
     import torch
     e, _ = eng.time_embedding()
     for _ in range(3):
@@ -709,12 +715,16 @@ def main():
     ap.add_argument("--skip-cpu", action="store_true", help="omit the cpu_baseline leg (debugging)")
     ap.add_argument("--workload", default="wan1.3b", choices=["wan1.3b", "wan14b", "flux", "hunyuan720p"],
                     help="wan14b: BASELINE configs[4] model/shape; flux: configs[0] (FLUX.1-dev 1024x1024, 28 steps); hunyuan720p: configs[3] "
-                         "(720p x 129 frames, 50 steps) — none of these is the driver's metric")
+                         "(720p x 129 frames, 50 steps) — none of these is the default metric")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the latent the last timed step returned as "
+                    "DIR/latent.npy (float32; Wan workloads)")
     args = ap.parse_args()
     select_workload(args.workload)
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
     if args.workload in ("flux", "hunyuan720p"):
+        if args.dump_outputs:
+            ap.error("--dump-outputs is implemented for the Wan workloads")
         run_mmdit(args, rank, world)
         return
     if args.impl == "reference":

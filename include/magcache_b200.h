@@ -1,11 +1,11 @@
 /*
- * magcache_b200 — C ABI of the B200-native MagCache hot path (libmagcache_b200.so).
+ * magcache_b200 — C ABI of the H100-native MagCache hot path (libmagcache_b200.so).
  *
  * Every entry point takes plain pointers and sizes (no torch types). Device pointers are raw CUDA device
  * addresses (tensor.data_ptr()); `stream` is a cudaStream_t passed as void* (torch.cuda.current_stream().cuda_stream).
  * All functions return 0 on success and a negative MC_ERR_* code on failure; mc_last_error() returns a
  * thread-local, human-readable description of the last failure. Nothing here falls back to the CPU:
- * device entry points fail with MC_ERR_CUDA if no sm_100 device/driver is usable.
+ * device entry points fail with MC_ERR_CUDA if no sm_90 device/driver is usable.
  *
  * Each declaration cites the reference statement(s) it replaces (paths relative to the Zehong-Ma/MagCache tree).
  */
@@ -232,7 +232,7 @@ int32_t mc_colmean_bf16(const void* x, int64_t ld, int32_t rows, int32_t cols, v
 /* y = silu(x), bf16 -> bf16 (fp32 inside): `self.silu(emb)` of AdaLayerNormZero / ...Single / ...Continuous. */
 int32_t mc_silu_bf16(const void* x, void* y, int64_t n, void* stream);
 
-/* bf16 GEMM on tcgen05/TMEM, TMA-fed:  acc[m,n] = sum_k A[m,k] * B[n,k]   (A: [M,K] row-major, B: [N,K] row-major).
+/* bf16 GEMM on wgmma, TMA-fed:  acc[m,n] = sum_k A[m,k] * B[n,k]   (A: [M,K] row-major, B: [N,K] row-major).
  * lda/ldb/ldo in elements; K % 8 == 0, lda % 8 == 0, ldb % 8 == 0, 16-byte aligned bases. */
 #define MC_EPI_BIAS_BF16 0        /* out_bf16[m,n] = bf16(acc + bias[n])                              nn.Linear under autocast */
 #define MC_EPI_BIAS_GELU_BF16 1   /* out_bf16 = bf16(gelu_tanh(float(bf16(acc + bias[n]))))            ffn[0] + GELU(tanh) */
@@ -246,7 +246,7 @@ int32_t mc_silu_bf16(const void* x, void* y, int64_t n, void* stream);
 int32_t mc_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t M, int32_t N, int32_t K,
                      const float* bias, int32_t epilogue, void* out, int64_t ldo, const float* gate, void* stream);
 
-/* Non-causal attention forward on tcgen05: out[i, h*128:(h+1)*128] = softmax(q_h k_h^T * scale) v_h, head_dim = 128
+/* Non-causal attention forward on wgmma: out[i, h*128:(h+1)*128] = softmax(q_h k_h^T * scale) v_h, head_dim = 128
  * (WanSelfAttention / WanT2VCrossAttention [EXT] behind MagCache4Wan2.1/magcache_generate.py:297-298; the joint attention of
  * MagCache4FLUX/magcache_flux.py:343-425 and MagCache4HunyuanVideo/magcache_sample_video.py:108-140).
  * q: [Lq, heads*128] bf16 (ldq), k: [Lk, heads*128] bf16 (ldk), v: [Lk, heads*128] bf16 (ldv) — all ROW-MAJOR views, so the three
@@ -308,8 +308,8 @@ int32_t mc_linear_f32_small(const float* x, int32_t M, int32_t K, const float* W
                             float* y, void* stream);
 
 /* Head + unpatchify (magcache_generate.py:304-305), with the cache-hit sum `x + residual_x` (:295) formed on the fly:
- * out[c, f, 2h+p, 2w+q] = Linear_fp32(LN(x)*(1+e1)+e0)[token, (p,q,c)], one pass over the rows (tcgen05, 3-pass bf16 split:
- * fp32-class accuracy; see csrc/head_tcgen05.cu).
+ * out[c, f, 2h+p, 2w+q] = Linear_fp32(LN(x)*(1+e1)+e0)[token, (p,q,c)], one pass over the rows (wgmma, 3-pass bf16 split:
+ * fp32-class accuracy; see csrc/head_wgmma.cu).
  * x: [rows, cols] for the tokens row_offset .. row_offset+rows-1 of the F*Hp*Wp grid (rows = F*Hp*Wp, row_offset = 0 unless the
  * token axis is sharded): fp32 with r == NULL (the residual stream), or bf16 together with r fp32 [rows, cols] — the
  * un-materialised hit sum x0_bf16 + r_f32. cols % 64 == 0.

@@ -1,4 +1,4 @@
-"""magcache_b200 — B200-native (sm_100a) MagCache denoising hot path behind the reference's monkey-patch API.
+"""magcache_b200 — H100-native (sm_90a) MagCache denoising hot path behind the reference's monkey-patch API.
 
     from magcache_b200 import magcache_forward, magcache_calibration, init_magcache
 

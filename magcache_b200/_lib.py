@@ -137,7 +137,7 @@ SIGNATURES = {
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} is missing: the CUDA extension has not been built. Run `python magcache_b200/build.py` "
-        "(needs nvcc; cross-compiles for sm_100a without a GPU). There is no CPU/eager fallback by design.")
+        "(needs nvcc; cross-compiles for sm_90a without a GPU). There is no CPU/eager fallback by design.")
 
 lib = ctypes.CDLL(LIB_PATH)
 lib.mc_last_error.restype = c_char_p

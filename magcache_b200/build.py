@@ -1,4 +1,4 @@
-"""Build libmagcache_b200.so (sm_100a only) in-tree with nvcc. `python magcache_b200/build.py [--force]`."""
+"""Build libmagcache_b200.so (sm_90a only) in-tree with nvcc. `python magcache_b200/build.py [--force]`."""
 import os
 import shutil
 import subprocess
@@ -7,8 +7,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmagcache_b200.so")
-SOURCES = ["controller.cu", "cache_kernels.cu", "rowwise_kernels.cu", "gemm_tcgen05.cu", "attn_tcgen05.cu", "head_tcgen05.cu", "p2p.cu", "dit_forward.cu", "nccl_gather.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
+SOURCES = ["controller.cu", "cache_kernels.cu", "rowwise_kernels.cu", "gemm_wgmma.cu", "attn_wgmma.cu", "head_wgmma.cu", "p2p.cu", "dit_forward.cu", "nccl_gather.cu"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
               "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
 
@@ -47,7 +47,7 @@ def build(force=False, verbose=False):
         f.write("\n".join(log))
     if verbose:
         print("\n".join(log))
-    cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static", "-ldl"]
+    cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static", "-ldl"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -1,7 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / st / fences) and the UMMA descriptors.
-// Bit layouts follow the PTX ISA "tcgen05 matrix/instruction descriptor" tables (the same ones
-// cute/arch/mma_sm100_desc.hpp encodes); nothing here depends on CUTLASS.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use: mbarrier, TMA (cp.async.bulk.tensor), wgmma and its
+// shared-memory matrix descriptors. Bit layouts follow the PTX ISA "matrix descriptor" table for wgmma; nothing here depends
+// on CUTLASS.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -42,7 +41,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Bounded wait: a pipeline bug must surface as a launch failure (trap), never as a hung GPU.
 #ifndef MC_MBAR_TIMEOUT_CYCLES
-#define MC_MBAR_TIMEOUT_CYCLES (4000000000ll)  // ~2 s at 1.9 GHz
+#define MC_MBAR_TIMEOUT_CYCLES (4000000000ll)  // ~2 s at 1.98 GHz
 #endif
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
@@ -56,11 +55,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// One lane of a fully converged warp. tcgen05.mma / commit and the TMA instructions take their operands from UNIFORM registers: under
-// a divergent `if (lane == 0)` ptxas has to wrap every one of them in a uniformisation loop (ELECT / PLOP3 / BRA.U.ANY, ~10
-// instructions and ~100 cycles per MMA — enough to make the single issuing thread the bottleneck of a kernel whose MMAs take 64
-// cycles each). Issued under elect.sync from warp-uniform control flow they are single instructions. The elected lane is the same on
-// every call (the lowest active one), which tcgen05.commit relies on.
+// One lane of a fully converged warp, for the single-thread TMA issue: elected from warp-uniform control flow, the copy
+// instructions take uniform operands without a uniformisation loop around them.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -76,11 +72,9 @@ __device__ __forceinline__ bool elect_one() {
 // ------------------------------------------------------------------------------------------------
 // proxies / fences
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void fence_proxy_async_smem() {  // generic-proxy smem writes -> visible to async proxy (UMMA/TMA)
+__device__ __forceinline__ void fence_proxy_async_smem() {  // generic-proxy smem writes -> visible to async proxy (wgmma/TMA)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------
 // TMA
@@ -104,120 +98,101 @@ __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gmem_sr
 }
 
 // ------------------------------------------------------------------------------------------------
-// TMEM allocation (one warp, .sync.aligned)
+// wgmma (warpgroup MMA, sm_90a): all 128 threads of a warpgroup issue each instruction; the fp32 accumulator lives in their
+// registers. Fragment of an m64nN accumulator: warp w of the warpgroup, lane l holds, for i in [0, N/8),
+//   d[4i + 0..1] = row 16w + l/4,     columns 8i + 2(l%4) + {0, 1}
+//   d[4i + 2..3] = row 16w + l/4 + 8, same columns
+// The register A operand of an m64k16 step (4 x bf16x2) follows the same pattern over 16 K columns:
+//   a[0] = (row, k 2(l%4)..+1)  a[1] = (row + 8, same k)  a[2] = (row, k 8 + 2(l%4)..+1)  a[3] = (row + 8, same k)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// UMMA descriptors
-// ------------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor for a K-major operand tile stored as [rows][64 bf16] (128-byte rows)
-// with the 128-byte swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B). 8-row groups are 1024 B apart (SBO).
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (unused for swizzled K-major; 1)
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1 (sm_100)      bits [61,64) layout = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128_kmajor(uint32_t smem_addr) {
+// Shared-memory matrix descriptor for a K-major operand tile stored as [rows][64 bf16] (128-byte rows) with the 128-byte
+// swizzle TMA writes (CU_TENSOR_MAP_SWIZZLE_128B). 8-row groups are 1024 B apart (SBO); one K16 step inside a row advances
+// the start address by 32 B (+2 in the >> 4 field).
+//   bits [0,14) start address >> 4   [16,30) leading byte offset >> 4 (unused for swizzled K-major; 1)
+//   bits [32,46) stride byte offset >> 4   [62,64) layout = 1 (SWIZZLE_128B)
+__device__ __forceinline__ uint64_t gmma_desc_sw128_kmajor(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// MN-major operand tile (the "N x K" B operand stored with N contiguous, e.g. V [kv, d] row-major for O += P V): TMA boxes of
-// [K rows][64 bf16] (128-byte rows, 128-byte swizzle). In 16-byte units the canonical layout is ((8,n),(8,k)):((1,LBO),(8,SBO)):
-// 64 MN-elements contiguous, the next 64 MN-elements LBO bytes further (= one TMA box), 8 K-rows 128 B apart, the next 8 K-rows
-// SBO = 1024 B further. One UMMA K-step (16 K-rows) advances the start address by 2048 B.
-__device__ __forceinline__ uint64_t umma_desc_sw128_mnmajor(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes = 1024) {
+// MN-major operand tile (the B operand of O += P V with V [kv, d] row-major, d contiguous): TMA boxes of [K rows][64 bf16]
+// (128-byte rows, 128-byte swizzle). 64 MN-elements contiguous, the next 64 MN-elements LBO bytes further (= one TMA box),
+// 8 K-rows 128 B apart, the next 8 K-rows SBO = 1024 B further. One K16 step advances the start address by 2048 B.
+__device__ __forceinline__ uint64_t gmma_desc_sw128_mnmajor(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes = 1024) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// Instruction descriptor, kind::f16: D fp32, A/B bf16, both K-major, dense, no negate.
-//   [4,6) D fmt (1=f32)  [7,10) A fmt (1=bf16)  [10,13) B fmt (1=bf16)  [15] A major (0=K)  [16] B major (0=K)
-//   [17,23) N>>3         [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_f32(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// same with the B operand MN-major (bit 16)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_f32_bmn(int M, int N) { return umma_idesc_bf16_f32(M, N) | (1u << 16); }
+// Keep the compiler from moving accesses of an accumulator across wgmma_fence / wgmma_wait (the asm above does not name it).
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread.
-__device__ __forceinline__ void umma_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+// D (+)= A[smem] * B[smem]^T, both K-major (generated: one wrapper per N the kernels use)
+__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// D[tmem] (+)= A[tmem] * B[smem]^T : A (bf16, K-major) lives in TMEM — lane = row, each 32-bit column holds two consecutive
-// K elements (16 bf16 of one UMMA_K step = 8 columns).
-__device__ __forceinline__ void umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// Arrive on an mbarrier when all tcgen05 async ops issued so far by this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void wgmma_m64n256k16_ss(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+// D (+)= A[registers] * B[smem], B MN-major (transposed)
+__device__ __forceinline__ void wgmma_m64n128k16_rs_tb(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %69, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "{%64, %65, %66, %67}, %68, p, 1, 1, 1;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
 
-// ------------------------------------------------------------------------------------------------
-// TMEM <-> registers. 32x32b: lane i of the warp reads TMEM lane (base_lane + i), N consecutive 32-bit columns.
-// taddr = (lane << 16) | column.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // Register reallocation between the warpgroups of a CTA (all 4 warps of a warpgroup execute it): the data-path warpgroups give
 // registers up, the compute warpgroups take them. N a multiple of 8 in [24, 256].
@@ -238,60 +213,19 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// Blackwell packed-fp32 and 3-input ALU ops (halve the issue slots of the softmax inner loop)
-__device__ __forceinline__ float max3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack_f32x2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-// 2^a, 2^b on the FMA / ALU pipes instead of the MUFU (FlashAttention-4's trick): Cody-Waite split x = floor(x) + f with the
-// magic-constant add rounded toward -inf, a cubic for 2^f on [0, 1) (max relative error 8.8e-5 — 22x below the bf16 rounding P
-// gets anyway), and the integer part added into the exponent field. 10 SASS instructions per PAIR (2 FMNMX, FADD2.RM, FADD2,
-// 4 FFMA2, 2 LEA) against 2 MUFU.EX2 that occupy the 16-lane special-function unit for 8 cycles per warp each.
-// Inputs below -126 (masked columns: -inf) give 2^-126 * [1, 2) instead of 0: finite, and below anything the row sum can see.
-__device__ __forceinline__ void ex2_emul_pair(float& a, float& b) {
+// 2^x on the FMA / ALU pipes instead of the MUFU: Cody-Waite split x = floor(x) + f with the magic-constant add rounded toward
+// -inf, a cubic for 2^f on [0, 1) (max relative error 8.8e-5, well below the bf16 rounding P gets anyway), and the integer part
+// added into the exponent field. Inputs below -126 (masked columns: -inf) give 2^-126 * [1, 2) instead of 0: finite, and below
+// anything the row sum can see.
+__device__ __forceinline__ float ex2_emul(float x) {
   const float kMagic = 12582912.0f;  // 1.5 * 2^23
-  a = fmaxf(a, -126.0f);
-  b = fmaxf(b, -126.0f);
-  uint64_t x2, t2, fi2, f2, p2;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(x2) : "f"(a), "f"(b));
-  uint64_t magic2, nmagic2, none2, c3, c2, c1, c0;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(magic2) : "f"(kMagic));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(nmagic2) : "f"(-kMagic));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(none2) : "f"(-1.0f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(c3) : "f"(0.077119089663028717041015625f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(c2) : "f"(0.227564394474029541015625f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(c1) : "f"(0.695146143436431884765625f));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(c0) : "f"(1.0f));
-  asm("add.rm.ftz.f32x2 %0, %1, %2;" : "=l"(t2) : "l"(x2), "l"(magic2));    // low mantissa bits of t = floor(x)
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(fi2) : "l"(t2), "l"(nmagic2));       // floor(x) as a float
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(f2) : "l"(fi2), "l"(none2), "l"(x2));  // f = x - floor(x) in [0, 1)
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(p2) : "l"(c3), "l"(f2), "l"(c2));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(p2) : "l"(p2), "l"(f2), "l"(c1));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(p2) : "l"(p2), "l"(f2), "l"(c0));
-  float ta, tb, pa, pb;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(ta), "=f"(tb) : "l"(t2));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(pa), "=f"(pb) : "l"(p2));
-  a = __int_as_float(__float_as_int(pa) + (__float_as_int(ta) << 23));
-  b = __int_as_float(__float_as_int(pb) + (__float_as_int(tb) << 23));
-}
-__device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  x = fmaxf(x, -126.0f);
+  const float t = __fadd_rd(x, kMagic);        // low mantissa bits of t = floor(x)
+  const float f = x - __fadd_rn(t, -kMagic);   // x - floor(x) in [0, 1)
+  float p = __fmaf_rn(0.077119089663028717041015625f, f, 0.227564394474029541015625f);
+  p = __fmaf_rn(p, f, 0.695146143436431884765625f);
+  p = __fmaf_rn(p, f, 1.0f);
+  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
 }
 __device__ __forceinline__ uint4 ld_nc_v4(const void* p) {  // streaming 128-bit load, no L1 allocation
   uint4 r;
@@ -302,22 +236,17 @@ __device__ __forceinline__ void st_na_v4(void* p, const uint4& v) {  // streamin
   asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
-// 256-bit global accesses (sm_100+): one instruction per lane moves 8 fp32, so a warp touches 1 KB contiguously and every
-// 32-byte sector is requested exactly once (two .v4 accesses per lane would request each sector twice from L2).
+// 8 fp32 per lane as two 128-bit accesses
 __device__ __forceinline__ void ld_nc_v8_f32(const float* p, float (&f)[8]) {
-  asm volatile("ld.global.nc.L1::no_allocate.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]), "=f"(f[4]), "=f"(f[5]), "=f"(f[6]), "=f"(f[7])
-               : "l"(p));
+  asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]) : "l"(p));
+  asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(f[4]), "=f"(f[5]), "=f"(f[6]), "=f"(f[7]) : "l"(p + 4));
 }
 __device__ __forceinline__ void ld_v8_f32(const float* p, float (&f)[8]) {  // coherent form: the buffer may be written by this kernel
-  asm volatile("ld.global.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]), "=f"(f[4]), "=f"(f[5]), "=f"(f[6]), "=f"(f[7])
-               : "l"(p)
-               : "memory");
+  asm volatile("ld.global.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(f[0]), "=f"(f[1]), "=f"(f[2]), "=f"(f[3]) : "l"(p) : "memory");
+  asm volatile("ld.global.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(f[4]), "=f"(f[5]), "=f"(f[6]), "=f"(f[7]) : "l"(p + 4) : "memory");
 }
 __device__ __forceinline__ void st_na_v8_f32(float* p, const float (&f)[8]) {
-  asm volatile("st.global.L1::no_allocate.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "f"(f[0]), "f"(f[1]), "f"(f[2]),
-               "f"(f[3]), "f"(f[4]), "f"(f[5]), "f"(f[6]), "f"(f[7])
-               : "memory");
+  asm volatile("st.global.L1::no_allocate.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(f[0]), "f"(f[1]), "f"(f[2]), "f"(f[3]) : "memory");
+  asm volatile("st.global.L1::no_allocate.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p + 4), "f"(f[4]), "f"(f[5]), "f"(f[6]), "f"(f[7]) : "memory");
 }
 }  // namespace ptx

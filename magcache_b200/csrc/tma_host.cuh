@@ -46,7 +46,7 @@ struct TmapCacheEntry {
   bool valid;
 };
 constexpr int kTmapCacheSize = 1024;
-TmapCacheEntry* tmap_cache();          // defined in gemm_tcgen05.cu (one table per process; entries are device-pointer keyed)
+TmapCacheEntry* tmap_cache();          // defined in gemm_wgmma.cu (one table per process; entries are device-pointer keyed)
 std::mutex& tmap_cache_mutex();
 
 inline int32_t make_tmap_bf16_2d_uncached(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows,

@@ -1,5 +1,5 @@
 """MMDiT engines (SURVEY §8f rank 4): the transformers behind `magcache_forward` of MagCache4FLUX/magcache_flux.py:234-440 (FLUX.1,
-FLUX.1-Kontext) and of MagCache4HunyuanVideo/magcache_sample_video.py:29-160 (HunyuanVideo) on the same sm_100a kernels as the Wan path — tcgen05 GEMMs (fused bias / GELU / SiLU / bf16 gated-residual epilogues), the tcgen05 flash
+FLUX.1-Kontext) and of MagCache4HunyuanVideo/magcache_sample_video.py:29-160 (HunyuanVideo) on the same sm_90a kernels as the Wan path — wgmma GEMMs (fused bias / GELU / SiLU / bf16 gated-residual epilogues), the wgmma flash
 attention over the joint text+image sequence, LN+modulate, per-head RMSNorm + RoPE, the K1/K2 cache kernels.
 
 Block arithmetic follows diffusers' `FluxTransformerBlock` / `FluxSingleTransformerBlock` and hyvideo's `MMDoubleStreamBlock` /
@@ -9,8 +9,8 @@ the forwards' own statements (embedders, controller, hit / miss, residual, final
 (`MMDiTCore`): same modulation chunk order, same per-head q/k RMSNorm, same `cat(attn, act(mlp))` single block; they differ in the
 token order of the joint sequence, in which rows get RoPE, and in their embedders.
 
-STATUS (end of round 1): parity-green on a B200 against the oracles at reduced depth / token counts (tests/test_flux_forward_gpu.py,
-tests/test_hunyuan_forward_gpu.py; profiles/r01_mmdit_first_gpu_run.md) and pinned on CPU through the kernel emulation
+STATUS (end of round 1): parity-green against the oracles at reduced depth / token counts (tests/test_flux_forward_gpu.py,
+tests/test_hunyuan_forward_gpu.py) and pinned on CPU through the kernel emulation
 (tests/test_*_engine_emulated_cpu.py); not yet run or timed at the full FLUX 1024^2 / HunyuanVideo 720p shapes. Nothing on the Wan path
 depends on this module.
 

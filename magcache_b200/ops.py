@@ -1,7 +1,7 @@
 """PyTorch-tensor front end of the C ABI: tensors in, tensors out, kernels on the current CUDA stream.
 
 PyTorch is used for device memory and streams only; every function below lands in exactly one hand-written
-sm_100a kernel of libmagcache_b200.so (see include/magcache_b200.h for the reference statement each one replaces).
+sm_90a kernel of libmagcache_b200.so (see include/magcache_b200.h for the reference statement each one replaces).
 """
 import math
 
@@ -285,7 +285,7 @@ def silu(x, out=None):
 
 
 def gemm(a, b, bias=None, epilogue=_lib.MC_EPI_BIAS_BF16, out=None, gate=None, tag=None):
-    """acc = a @ b.T on tcgen05 (a [M,K] bf16, b [N,K] bf16, row stride allowed) + fused epilogue (see MC_EPI_*)."""
+    """acc = a @ b.T on wgmma (a [M,K] bf16, b [N,K] bf16, row stride allowed) + fused epilogue (see MC_EPI_*)."""
     _dev(a), _dev(b)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and a.stride(1) == 1 and b.stride(1) == 1
     M, K = a.shape

@@ -107,7 +107,7 @@ def _sync_slot_in(self, eng, slot):
 
 
 def magcache_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
-    r"""MagCache4Wan2.1/magcache_generate.py:198-312 on the B200 kernels.
+    r"""MagCache4Wan2.1/magcache_generate.py:198-312 on the H100 kernels.
 
     Args / returns as the reference: x List[Tensor[C_in, F, H, W]], t Tensor[B], context List[Tensor[L, C]], seq_len int
     -> List[Tensor[C_out, F, H, W]] (float32).
@@ -354,7 +354,7 @@ class _Sample:
 def magcache_flux_forward(self, hidden_states, encoder_hidden_states=None, pooled_projections=None, timestep=None, img_ids=None,
                           txt_ids=None, guidance=None, joint_attention_kwargs=None, controlnet_block_samples=None,
                           controlnet_single_block_samples=None, return_dict=True, controlnet_blocks_repeat=False):
-    r"""MagCache4FLUX/magcache_flux.py:234-440 on the B200 kernels: same signature, same state attributes (`cnt, num_steps,
+    r"""MagCache4FLUX/magcache_flux.py:234-440 on the H100 kernels: same signature, same state attributes (`cnt, num_steps,
     magcache_thresh, K, retention_ratio, accumulated_ratio / _err / _steps, previous_residual, mag_ratios`), `(output,)` or an object
     with `.sample`. LoRA scaling, ip-adapter and ControlNet residuals (:275-288, :321-324, :371-381, :410-420) are not built and raise."""
     if joint_attention_kwargs or controlnet_block_samples is not None or controlnet_single_block_samples is not None:
@@ -465,7 +465,7 @@ def init_magcache_flux(transformer, num_inference_steps=28, thresh=0.24, K=5, re
 
 def magcache_hunyuan_forward(self, x, t, text_states=None, text_mask=None, text_states_2=None, freqs_cos=None, freqs_sin=None,
                              guidance=None, return_dict=True):
-    r"""MagCache4HunyuanVideo/magcache_sample_video.py:29-160 on the B200 kernels (MMDiT engine, magcache_b200/mmdit.py; opt-in until
+    r"""MagCache4HunyuanVideo/magcache_sample_video.py:29-160 on the H100 kernels (MMDiT engine, magcache_b200/mmdit.py; opt-in until
     validated on a GPU): same signature and state attributes (`cnt, num_steps, magcache_thresh, K, retention_ratio, accumulated_ratio /
     _err / _steps, residual_cache, mag_ratios`), returns `{"x": img}` or the tensor. x [1, 16, T, H, W]; text_mask marks the valid
     (right-padded) text tokens."""
@@ -565,7 +565,7 @@ def init_magcache_hunyuan(transformer, infer_steps=50, thresh=0.24, K=6, retenti
 # The paper-evaluation variant of the Wan forward (the code behind the published Wan2.1 numbers)
 # ------------------------------------------------------------------------------------------------------------------
 def magcache_eval_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
-    r"""eval/magcache/experiments/Wan2.1_EVAL/wan_magcache.py:682-817 on the B200 kernels, state under THAT script's attribute
+    r"""eval/magcache/experiments/Wan2.1_EVAL/wan_magcache.py:682-817 on the H100 kernels, state under THAT script's attribute
     names (`t, num_steps, magcache_thresh, magcache_K, ratio, accumulated_sim, accumulated_err, accumulated_steps, residual_cache,
     skip_steps, pre_con`). Differences from `magcache_forward`, all reproduced: `<=` threshold compare, table indexed `ratio[t-10]`,
     retention fixed at `int(num_steps*0.2)`, residuals kept from call 10 on (`cache_time`) in a `[2, B, N, D, 1]` tensor — the
@@ -655,7 +655,7 @@ def _tea_structs(self):
 
 
 def teacache_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
-    r"""eval/magcache/experiments/Wan2.1_EVAL/wan_teacache.py:457-590 on the B200 kernels, state under the reference's attribute
+    r"""eval/magcache/experiments/Wan2.1_EVAL/wan_teacache.py:457-590 on the H100 kernels, state under the reference's attribute
     names (`cnt, num_steps, teacache_thresh, accumulated_rel_l1_distance_even/odd, previous_e0_even/odd,
     previous_residual_even/odd, use_ref_steps, ret_steps, cutoff_steps, coefficients, enable_teacache`). The decision reads the
     relative L1 change of the modulated time embedding (one tiny reduction + the `.item()` sync the reference has), the hit /

@@ -3,7 +3,7 @@
 Everything in the forward is token-local except self-attention, which needs every key/value. Each rank owns a contiguous
 range of tokens (contiguous in (f, h, w) raster order — the "temporal/token shard"), keeps its slice of the residual stream
 and of the residual cache (as the reference's only sequence-parallel MagCache does, eval/magcache/experiments/opensora.py:310,347),
-and per layer contributes its K|V rows to the other ranks — the B200 counterpart of videosys/core/comm.py:272-292
+and per layer contributes its K|V rows to the other ranks — the counterpart of videosys/core/comm.py:272-292
 (`dist.all_gather` + `torch.cat`). The controller is a pure function of `cnt` and the table, so every rank takes the same
 hit/miss decision without communicating.
 

@@ -1,4 +1,4 @@
-"""Wan2.1 DiT engine: device-resident weights in the layout the sm_100a kernels want, plus the kernel sequence of one forward.
+"""Wan2.1 DiT engine: device-resident weights in the layout the sm_90a kernels want, plus the kernel sequence of one forward.
 
 This is the cache-miss branch of the reference (`for block in self.blocks: x = block(x, **kwargs)`,
 MagCache4Wan2.1/magcache_generate.py:297-298) and the prologue / epilogue around it (:229-275, :304-305), rebuilt on the

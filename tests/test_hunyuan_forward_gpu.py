@@ -1,8 +1,7 @@
 """HunyuanVideo MMDiT engine on the GPU: `magcache_hunyuan_forward` against the oracle restatement of
 MagCache4HunyuanVideo/magcache_sample_video.py:29-160, and the column-mean kernel against torch.
 
-First B200 run (end of round 1): all green — ours vs oracle 4.8e-3 rel-L2, ours vs fp64 5.39e-3 against the bf16 oracle's own 5.88e-3
-(profiles/r01_mmdit_first_gpu_run.md). The orchestration is also pinned on CPU through the kernel emulation
+The orchestration is also pinned on CPU through the kernel emulation
 (tests/test_hunyuan_engine_emulated_cpu.py)."""
 import copy
 import os

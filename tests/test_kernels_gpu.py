@@ -453,7 +453,7 @@ def test_head_unpatchify(fused):
     assert torch.allclose(out, ref, rtol=1e-3, atol=1e-4), float((out - ref).abs().max())
 
 
-# ------------------------------------------------------------------------------------------- tcgen05 GEMM
+# ------------------------------------------------------------------------------------------- wgmma GEMM
 def _gemm_ref(a, b):
     return a.double() @ b.double().t()
 
@@ -571,7 +571,7 @@ def test_rmsnorm_rope_staged_form_matches_register_form_bitwise():
     assert torch.equal(ya[:1000], yb)
 
 
-# ------------------------------------------------------------------------------------------- tcgen05 attention
+# ------------------------------------------------------------------------------------------- wgmma attention
 def _attn_ref(q, k, v, heads):
     Lq, W = q.shape
     qh = q.double().view(Lq, heads, 128).transpose(0, 1)
@@ -602,9 +602,9 @@ def test_attention(Lq, Lk, heads, qscale):
 @pytest.mark.parametrize("Lq,Lk,heads,qscale", [(128, 128, 1, 1.0), (256, 256, 1, 1.0), (300, 1000, 3, 1.0), (513, 1285, 2, 6.0), (1000, 4095, 12, 1.0),
                                                 (40, 130, 1, 3.0)])
 def test_attention_long_kernel(Lq, Lk, heads, qscale, emu, monkeypatch):
-    """The 256-row / 128-wide-KV kernel forced onto small and ragged shapes (second query tile empty or partial, one KV tile, ragged
-    last KV tile), for every exponential-emulation fraction it is built with: same bounds as the default path, and each variant
-    bit-reproducible."""
+    """The 128-wide-KV instantiation forced onto small and ragged shapes (second consumer warpgroup's rows empty or partial, one KV
+    tile, ragged last KV tile), for every exponential-emulation fraction it is built with: same bounds as the default path, and each
+    variant bit-reproducible."""
     ops = _ops()
     monkeypatch.setenv("MC_ATTN_KERNEL", "2")
     monkeypatch.setenv("MC_ATTN_EMU", str(emu))

@@ -1,9 +1,9 @@
-"""End-to-end parity of the B200 path (called exactly as the reference calls it: `model.forward = magcache_forward` + class
+"""End-to-end parity of the H100 path (called exactly as the reference calls it: `model.forward = magcache_forward` + class
 attributes) against the CPU oracle restatement of MagCache4Wan2.1/magcache_generate.py:198-312 on identical synthetic latents,
 timesteps, text embeddings and weights.
 
 Tolerances. The skip mask / controller state: bit-exact. Tensors: both implementations run bf16 GEMMs with fp32 accumulation
-but sum in different orders (MKL/oneDNN vs tcgen05), so individual bf16 roundings flip by one ulp and the difference grows
+but sum in different orders (MKL/oneDNN vs wgmma), so individual bf16 roundings flip by one ulp and the difference grows
 with depth; an element-wise rtol 1e-3 is not meaningful for a bf16 pipeline. We therefore check (a) relative L2 error of our
 output against the oracle <= 2e-2, and (b) the north-star criterion in the only form that is well defined: our error against
 an fp64 evaluation of the same network is no larger than 1.5x the bf16 oracle's own error against it (+1e-4 absolute).
