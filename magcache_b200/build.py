@@ -47,6 +47,13 @@ def build(force=False, verbose=False):
         f.write("\n".join(log))
     if verbose:
         print("\n".join(log))
+    # C7510: ptxas serialised a kernel's wgmmas (a wait after every one) because the kernel contains a function call, e.g. a
+    # device printf. That silently costs the tensor-core kernels a large part of their rate, so it is a build error.
+    serialised = [line.strip() for line in "\n".join(log).splitlines() if "C7510" in line]
+    if serialised:
+        raise RuntimeError("ptxas serialised wgmma (C7510); no kernel that issues wgmma may contain a function call such as "
+                           "device printf (see MC_DEVICE_DIAG in csrc/ptx.cuh). Full log: build/ptxas.log\n" +
+                           "\n".join(serialised[:8]))
     cmd = [_nvcc(), "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static", "-ldl"]
     subprocess.check_call(cmd)
     return LIB

@@ -14,6 +14,8 @@
 //   warpgroups 1-2  consumers, 64 query rows each: S = Q K^T (wgmma, both operands in shared memory) into registers, online
 //                   softmax in the exp2 domain on the accumulator fragment (a row spans the 4 lanes of a quad), P rounded to bf16
 //                   and fed back as the REGISTER A operand of O += P V, O in registers.
+//                   The two warpgroups take turns issuing their GEMMs (ping-pong on named barriers), so one's softmax runs
+//                   while the tensor cores work on the other's GEMM.
 // The units of a partially filled last wave are split over the KV range and merged by attn_combine_kernel.
 // The 128-key variant can evaluate a fixed fraction of the softmax exponentials on the FMA pipe (ptx::ex2_emul) instead of the
 // MUFU unit; MC_ATTN_EMU selects the fraction per call.
@@ -99,7 +101,7 @@ __device__ __forceinline__ void wait_segments(const AttnParams& p, int row0, int
       if (static_cast<int32_t>(v - want) >= 0) break;
       __nanosleep(100);
       if (clock64() - t0 > MC_MBAR_TIMEOUT_CYCLES) {
-        printf("attention: key segment %d never arrived (flag %u, epoch %u)\n", s, v, want);
+        MC_DIAG("attention: key segment %d never arrived (flag %u, epoch %u)\n", s, v, want);
         __trap();
       }
     }
@@ -152,7 +154,7 @@ __global__ void __launch_bounds__(ak::kThreads, 1)
 
   if (threadIdx.x == 0) {
     if ((ptx::smem_u32(smem) & 1023u) != 0) {
-      printf("attn_kernel: dynamic smem base not 1024-aligned\n");
+      MC_DIAG("attn_kernel: dynamic smem base not 1024-aligned\n");
       __trap();
     }
     ptx::prefetch_tmap(&tmap_q);
@@ -224,11 +226,28 @@ __global__ void __launch_bounds__(ak::kThreads, 1)
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;  // rows r and r + 8 (l: this thread's columns only)
     ptx::mbar_wait(q_full, 0);
 
-    for (int j = 0; j < n_tiles; ++j) {
+    // Each warpgroup runs the serial flash-attention recurrence per KV tile j: S(j) = Q K(j)^T, online softmax, O += P(j) V(j).
+    // (Issuing S(j) and PV(j-1) back to back within a warpgroup needs O, S and P live across the wait, ~170 registers with
+    // addressing; ptxas allocates this kernel's consumers 168 despite setmaxnreg and then spills and serialises the wgmmas.)
+    //
+    // Ping-pong between the two consumer warpgroups instead: warpgroup w issues each GEMM (S(j), then PV(j)) only between
+    // bar.sync on barrier 1 + w and bar.arrive on the other's barrier 2 - w, so issue alternates S0 S1 PV0 PV1 S0 ... and one
+    // warpgroup's softmax runs while the tensor cores work through the other's GEMM. Both warpgroups run the same 2 n_tiles
+    // turns whatever rows they hold (a warpgroup whose rows are past Lq computes on TMA's zero fill), since n_tiles is uniform
+    // over the CTA. Warpgroup 0 pre-arrives once on its own barrier and warpgroup 1 skips its arrival after its last turn, so
+    // on each barrier the arrivals equal the syncs (2 n_tiles) and both are at rest when the CTA exits. The K/V mbarrier waits
+    // come before a turn is taken, never inside one, so a warpgroup holding the turn never waits on the producer.
+    constexpr uint32_t kTurnThreads = 256;
+    const uint32_t bar_own = 1 + wg, bar_other = 2 - wg;
+    auto turn_begin = [&] { ptx::named_bar_sync(bar_own, kTurnThreads); };
+    auto turn_end = [&] { ptx::named_bar_arrive(bar_other, kTurnThreads); };
+    if (wg == 0) ptx::named_bar_arrive(bar_own, kTurnThreads);
+
+    float sc[BKV / 2];
+    uint32_t pa[BKV / 16][4];  // P of the tile whose PV is issued next, as the register A operand
+    const int valid = p.Lk - (total_tiles - 1) * BKV;
+    auto issue_s = [&](int j) {
       const int s = j & 1;
-      const uint32_t ph = (j >> 1) & 1;
-      float sc[BKV / 2];
-      ptx::mbar_wait(&k_full[s], ph);
       ptx::wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < kHD / 16; ++kk) {
@@ -242,12 +261,24 @@ __global__ void __launch_bounds__(ak::kThreads, 1)
         }
       }
       ptx::wgmma_commit();
-      ptx::wgmma_wait<0>();
+    };
+    auto issue_pv = [&](int j) {
+      const int s = j & 1;
+      ptx::fence_regs(o);
+      ptx::wgmma_fence();
+      const uint64_t dv = ptx::gmma_desc_sw128_mnmajor(v_base + s * L::kVBytes, BKV * 128);  // LBO = one [BKV kv x 64 d] box
+#pragma unroll
+      for (int kk = 0; kk < BKV / 16; ++kk)  // one K16 step = 16 kv rows = 2048 B of the MN-major tile
+        ptx::wgmma_m64n128k16_rs_tb(o, pa[kk], dv + static_cast<uint64_t>(kk * (2048 / 16)), 1u);
+      ptx::wgmma_commit();
+    };
+    // S(j) has retired (the caller's wgmma_wait): hand K(j) back, then the online softmax of tile j, P(j) in fp32 in place of
+    // S(j); returns the factors O is scaled by
+    auto softmax = [&](int j, float& f0, float& f1) {
       ptx::fence_regs(sc);
       __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&k_empty[s]);
+      if (lane == 0) ptx::mbar_arrive(&k_empty[j & 1]);
       if (j == j_ragged) {  // keys past Lk (zero-filled by TMA) must not take part in the softmax
-        const int valid = p.Lk - (total_tiles - 1) * BKV;
 #pragma unroll
         for (int i = 0; i < BKV / 8; ++i)
 #pragma unroll
@@ -267,39 +298,57 @@ __global__ void __launch_bounds__(ak::kThreads, 1)
         mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, off));
       }
       const float mn0 = fmaxf(m0, mx0 * p.scale_log2), mn1 = fmaxf(m1, mx1 * p.scale_log2);
-      const float f0 = ptx::ex2_approx(m0 - mn0), f1 = ptx::ex2_approx(m1 - mn1);  // 0 on the first tile (m = -inf)
+      f0 = ptx::ex2_approx(m0 - mn0), f1 = ptx::ex2_approx(m1 - mn1);  // 0 on the first tile (m = -inf)
       m0 = mn0, m1 = mn1;
       l0 *= f0, l1 *= f1;
+      // P = 2^(s*scale - m), row sum in fp32 before the bf16 rounding (as flash-attention does)
+#pragma unroll
+      for (int i = 0; i < BKV / 8; ++i) {
+        sc[4 * i] = exp2_sel<EMU_MASK>(fmaf(sc[4 * i], p.scale_log2, -m0), i);
+        sc[4 * i + 1] = exp2_sel<EMU_MASK>(fmaf(sc[4 * i + 1], p.scale_log2, -m0), i);
+        sc[4 * i + 2] = exp2_sel<EMU_MASK>(fmaf(sc[4 * i + 2], p.scale_log2, -m1), i);
+        sc[4 * i + 3] = exp2_sel<EMU_MASK>(fmaf(sc[4 * i + 3], p.scale_log2, -m1), i);
+        l0 += sc[4 * i] + sc[4 * i + 1];
+        l1 += sc[4 * i + 2] + sc[4 * i + 3];
+      }
+    };
+    // P(j) rounded to bf16 and packed as the A operand
+    auto pack_p = [&] {
+#pragma unroll
+      for (int i = 0; i < BKV / 8; ++i) {
+        pa[i >> 1][(i & 1) * 2] = pack_bf16x2(sc[4 * i], sc[4 * i + 1]);
+        pa[i >> 1][(i & 1) * 2 + 1] = pack_bf16x2(sc[4 * i + 2], sc[4 * i + 3]);
+      }
+    };
+    // PV(j) has retired (the caller's wgmma_wait<0>): hand V(j) back
+    auto release_v = [&](int j) {
+      ptx::fence_regs(o);
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&v_empty[j & 1]);
+    };
+    auto rescale_o = [&](float f0, float f1) {
 #pragma unroll
       for (int i = 0; i < kHD / 8; ++i) {
         o[4 * i] *= f0, o[4 * i + 1] *= f0;
         o[4 * i + 2] *= f1, o[4 * i + 3] *= f1;
       }
-      // P = 2^(s*scale - m), row sum in fp32 before the bf16 rounding (as flash-attention does), packed as the A operand
-      uint32_t pa[BKV / 16][4];
-#pragma unroll
-      for (int i = 0; i < BKV / 8; ++i) {
-        const float p0 = exp2_sel<EMU_MASK>(fmaf(sc[4 * i], p.scale_log2, -m0), i);
-        const float p1 = exp2_sel<EMU_MASK>(fmaf(sc[4 * i + 1], p.scale_log2, -m0), i);
-        const float p2 = exp2_sel<EMU_MASK>(fmaf(sc[4 * i + 2], p.scale_log2, -m1), i);
-        const float p3 = exp2_sel<EMU_MASK>(fmaf(sc[4 * i + 3], p.scale_log2, -m1), i);
-        l0 += p0 + p1;
-        l1 += p2 + p3;
-        pa[i >> 1][(i & 1) * 2] = pack_bf16x2(p0, p1);
-        pa[i >> 1][(i & 1) * 2 + 1] = pack_bf16x2(p2, p3);
-      }
-      ptx::mbar_wait(&v_full[s], ph);
-      ptx::fence_regs(o);
-      ptx::wgmma_fence();
-      const uint64_t dv = ptx::gmma_desc_sw128_mnmajor(v_base + s * L::kVBytes, BKV * 128);  // LBO = one [BKV kv x 64 d] box
-#pragma unroll
-      for (int kk = 0; kk < BKV / 16; ++kk)  // one K16 step = 16 kv rows = 2048 B of the MN-major tile
-        ptx::wgmma_m64n128k16_rs_tb(o, pa[kk], dv + static_cast<uint64_t>(kk * (2048 / 16)), 1u);
-      ptx::wgmma_commit();
+    };
+    for (int j = 0; j < n_tiles; ++j) {
+      ptx::mbar_wait(&k_full[j & 1], (j >> 1) & 1);
+      turn_begin();
+      issue_s(j);
+      turn_end();
       ptx::wgmma_wait<0>();
-      ptx::fence_regs(o);
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&v_empty[s]);
+      float f0, f1;
+      softmax(j, f0, f1);
+      rescale_o(f0, f1);
+      pack_p();
+      ptx::mbar_wait(&v_full[j & 1], (j >> 1) & 1);
+      turn_begin();
+      issue_pv(j);
+      if (wg == 0 || j + 1 < n_tiles) turn_end();  // warpgroup 1's last turn has no successor to release
+      ptx::wgmma_wait<0>();
+      release_v(j);
     }
 
     // ---- epilogue: O / l -> bf16 -> global (or the normalised fp32 partial of this split)

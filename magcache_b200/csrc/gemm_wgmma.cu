@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 
   if (threadIdx.x == 0) {
     if ((ptx::smem_u32(smem) & 1023u) != 0) {
-      printf("gemm_bf16_kernel: dynamic smem base not 1024-aligned\n");
+      MC_DIAG("gemm_bf16_kernel: dynamic smem base not 1024-aligned\n");
       __trap();
     }
     ptx::prefetch_tmap(&tmap_a);

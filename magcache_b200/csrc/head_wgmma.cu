@@ -155,7 +155,7 @@ __global__ void __launch_bounds__(hd::kThreads, 1) head_tc_kernel(const __grid_c
 
   if (threadIdx.x == 0) {
     if ((ptx::smem_u32(smem) & 1023u) != 0) {
-      printf("head_tc_kernel: dynamic smem base not 1024-aligned\n");
+      MC_DIAG("head_tc_kernel: dynamic smem base not 1024-aligned\n");
       __trap();
     }
     ptx::prefetch_tmap(&maps.f32_full);

@@ -39,6 +39,19 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
+// Device-side diagnostics before a __trap(). Device printf compiles to a call to vprintf, and ptxas cannot keep a wgmma
+// pipeline open across a function call: any kernel that issues wgmma and contains a printf on ANY path gets every wgmma
+// serialised (ptxas C7510, a wait after each instruction). So the messages are compiled out by default and the traps alone
+// remain; -DMC_DEVICE_DIAG=1 brings them back for a local debug build, at that cost (build.py rejects C7510 otherwise).
+#ifndef MC_DEVICE_DIAG
+#define MC_DEVICE_DIAG 0
+#endif
+#if MC_DEVICE_DIAG
+#define MC_DIAG(...) printf(__VA_ARGS__)
+#else
+#define MC_DIAG(...) ((void)0)
+#endif
+
 // Bounded wait: a pipeline bug must surface as a launch failure (trap), never as a hung GPU.
 #ifndef MC_MBAR_TIMEOUT_CYCLES
 #define MC_MBAR_TIMEOUT_CYCLES (4000000000ll)  // ~2 s at 1.98 GHz
@@ -48,11 +61,21 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
     if (clock64() - t0 > MC_MBAR_TIMEOUT_CYCLES) {
-      printf("mbar_wait timeout: block (%d,%d,%d) thread %d bar smem+%u parity %u\n", blockIdx.x, blockIdx.y, blockIdx.z,
-             threadIdx.x, smem_u32(bar), parity);
+      MC_DIAG("mbar_wait timeout: block (%d,%d,%d) thread %d bar smem+%u parity %u\n", blockIdx.x, blockIdx.y, blockIdx.z,
+              threadIdx.x, smem_u32(bar), parity);
       __trap();
     }
   }
+}
+
+// Named barriers (bar.sync / bar.arrive with an explicit id and thread count, a multiple of 32). Id 0 is __syncthreads'.
+// bar.arrive does not wait; bar.sync waits until `count` threads have arrived or synced on `id`. No timeout exists for these:
+// callers must make every arrival pair with a sync by construction.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
 // One lane of a fully converged warp, for the single-thread TMA issue: elected from warp-uniform control flow, the copy
