@@ -224,19 +224,24 @@ __global__ void __launch_bounds__(ak::kThreads, 1)
 #pragma unroll
     for (int i = 0; i < kHD / 2; ++i) o[i] = 0.f;
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;  // rows r and r + 8 (l: this thread's columns only)
-    ptx::mbar_wait(q_full, 0);
+    // The consumer's mbarrier waits record a timeout instead of trapping (ptx::mbar_wait_or_flag: a trap on them makes
+    // ptxas spill P and serialise the wgmmas of the pipelined loop below); the trap comes after the last wgmma_wait.
+    bool timed_out = false;
+    ptx::mbar_wait_or_flag(q_full, 0, timed_out);
 
-    // Each warpgroup runs the serial flash-attention recurrence per KV tile j: S(j) = Q K(j)^T, online softmax, O += P(j) V(j).
-    // (Issuing S(j) and PV(j-1) back to back within a warpgroup needs O, S and P live across the wait, ~170 registers with
-    // addressing; ptxas allocates this kernel's consumers 168 despite setmaxnreg and then spills and serialises the wgmmas.)
+    // Each warpgroup runs the flash-attention recurrence per KV tile j: S(j) = Q K(j)^T, online softmax, O = f(j) O + P(j) V(j),
+    // software-pipelined by one tile: S(j) and PV(j-1) are issued back to back, the softmax of tile j runs while PV(j-1) is on
+    // the tensor cores, then O is rescaled by f(j) and P(j) packed for the next turn. Every row still sees rescale by f(j),
+    // then + P(j) V(j), in tile order, so the result is bit-identical to the serial loop. Live across the wait: O (64 fp32),
+    // S(j) (BKV / 2 fp32) and P(j-1) (BKV / 4 packed bf16x2), ~160 registers for 128-key tiles, within setmaxnreg's 240.
     //
-    // Ping-pong between the two consumer warpgroups instead: warpgroup w issues each GEMM (S(j), then PV(j)) only between
-    // bar.sync on barrier 1 + w and bar.arrive on the other's barrier 2 - w, so issue alternates S0 S1 PV0 PV1 S0 ... and one
-    // warpgroup's softmax runs while the tensor cores work through the other's GEMM. Both warpgroups run the same 2 n_tiles
-    // turns whatever rows they hold (a warpgroup whose rows are past Lq computes on TMA's zero fill), since n_tiles is uniform
-    // over the CTA. Warpgroup 0 pre-arrives once on its own barrier and warpgroup 1 skips its arrival after its last turn, so
-    // on each barrier the arrivals equal the syncs (2 n_tiles) and both are at rest when the CTA exits. The K/V mbarrier waits
-    // come before a turn is taken, never inside one, so a warpgroup holding the turn never waits on the producer.
+    // The two consumer warpgroups also take turns: warpgroup w issues its GEMMs only between bar.sync on barrier 1 + w and
+    // bar.arrive on the other's barrier 2 - w, so one warpgroup's softmax runs while the tensor cores work through the other's
+    // GEMMs. Each warpgroup makes n_tiles + 1 turns (S(0); S(j) + PV(j-1) for j in [1, n_tiles); PV(n_tiles-1)) whatever rows
+    // it holds (a warpgroup whose rows are past Lq computes on TMA's zero fill), since n_tiles is uniform over the CTA.
+    // Warpgroup 0 pre-arrives once on its own barrier and warpgroup 1 skips its arrival after its last turn, so on each
+    // barrier the arrivals equal the syncs (n_tiles + 1) and both are at rest when the CTA exits. The K/V mbarrier waits come
+    // before a turn is taken, never inside one, so a warpgroup holding the turn never waits on the producer.
     constexpr uint32_t kTurnThreads = 256;
     const uint32_t bar_own = 1 + wg, bar_other = 2 - wg;
     auto turn_begin = [&] { ptx::named_bar_sync(bar_own, kTurnThreads); };
@@ -333,23 +338,42 @@ __global__ void __launch_bounds__(ak::kThreads, 1)
         o[4 * i + 2] *= f1, o[4 * i + 3] *= f1;
       }
     };
-    for (int j = 0; j < n_tiles; ++j) {
-      ptx::mbar_wait(&k_full[j & 1], (j >> 1) & 1);
+    {  // prologue: S(0), its softmax and P(0)
+      ptx::mbar_wait_or_flag(&k_full[0], 0, timed_out);
       turn_begin();
-      issue_s(j);
+      issue_s(0);
       turn_end();
       ptx::wgmma_wait<0>();
       float f0, f1;
-      softmax(j, f0, f1);
+      softmax(0, f0, f1);
       rescale_o(f0, f1);
       pack_p();
-      ptx::mbar_wait(&v_full[j & 1], (j >> 1) & 1);
+    }
+    for (int j = 1; j < n_tiles; ++j) {  // steady state: S(j) and PV(j-1) in one turn, softmax(j) under PV(j-1)
+      ptx::mbar_wait_or_flag(&k_full[j & 1], (j >> 1) & 1, timed_out);
+      ptx::mbar_wait_or_flag(&v_full[(j - 1) & 1], ((j - 1) >> 1) & 1, timed_out);
+      turn_begin();
+      issue_s(j);
+      issue_pv(j - 1);
+      turn_end();
+      ptx::wgmma_wait<1>();  // S(j) has retired, PV(j-1) may still run
+      float f0, f1;
+      softmax(j, f0, f1);
+      ptx::wgmma_wait<0>();
+      release_v(j - 1);
+      rescale_o(f0, f1);
+      pack_p();
+    }
+    {  // epilogue: PV(n-1)
+      const int j = n_tiles - 1;
+      ptx::mbar_wait_or_flag(&v_full[j & 1], (j >> 1) & 1, timed_out);
       turn_begin();
       issue_pv(j);
-      if (wg == 0 || j + 1 < n_tiles) turn_end();  // warpgroup 1's last turn has no successor to release
+      if (wg == 0) turn_end();  // warpgroup 1's last turn has no successor to release
       ptx::wgmma_wait<0>();
       release_v(j);
     }
+    if (timed_out) __trap();
 
     // ---- epilogue: O / l -> bf16 -> global (or the normalised fp32 partial of this split)
 #pragma unroll

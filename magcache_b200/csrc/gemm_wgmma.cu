@@ -50,6 +50,7 @@ struct GemmParams {
   void* out;
   int64_t ldo;
   const float* gate;
+  int total_tiles;  // m tiles x n tiles, set by launch_gemm_bn: read from the parameter bank, the loop bound costs no register
 };
 
 // One 32-row x 32-column patch: `stage` holds acc[r][c] at stage[r*33 + c]; lane = column. All global accesses below
@@ -66,17 +67,22 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
     const float b = (p.bias && col_ok) ? p.bias[col] : 0.f;
     const float g = (p.gate && col_ok) ? p.gate[col] : 1.f;
     float* xcol = static_cast<float*>(p.out) + static_cast<int64_t>(row0) * p.ldo + col;
-    float xv[32];
+    // two halves of 16 rows, 16 loads in flight each: all 32 rows at once spilled next to the 256-wide tile's 128 accumulator
+    // registers (same operations per element, same order)
 #pragma unroll
-    for (int r = 0; r < 32; ++r) xv[r] = (col_ok && r < rows) ? xcol[static_cast<int64_t>(r) * p.ldo] : 0.f;  // 32 loads in flight
+    for (int h = 0; h < 32; h += 16) {
+      float xv[16];
 #pragma unroll
-    for (int r = 0; r < 32; ++r) {
-      const float y = round_bf16(stage[r * kStagePad + lane] + b);
-      xv[r] = __fadd_rn(xv[r], __fmul_rn(y, g));
+      for (int r = 0; r < 16; ++r) xv[r] = (col_ok && h + r < rows) ? xcol[static_cast<int64_t>(h + r) * p.ldo] : 0.f;
+#pragma unroll
+      for (int r = 0; r < 16; ++r) {
+        const float y = round_bf16(stage[(h + r) * kStagePad + lane] + b);
+        xv[r] = __fadd_rn(xv[r], __fmul_rn(y, g));
+      }
+#pragma unroll
+      for (int r = 0; r < 16; ++r)
+        if (col_ok && h + r < rows) xcol[static_cast<int64_t>(h + r) * p.ldo] = xv[r];
     }
-#pragma unroll
-    for (int r = 0; r < 32; ++r)
-      if (col_ok && r < rows) xcol[static_cast<int64_t>(r) * p.ldo] = xv[r];
     return;
   }
 
@@ -194,8 +200,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   uint64_t* empty_bar = full_bar + kStages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m_tiles = (p.M + kBM - 1) / kBM, n_tiles = (p.N + kBN - 1) / kBN;
-  const int total_tiles = m_tiles * n_tiles;
+  const int n_tiles = (p.N + kBN - 1) / kBN;
+  const int total_tiles = p.total_tiles;
   const int num_kb = (p.K + kBK - 1) / kBK;
 
   if (threadIdx.x == 0) {
@@ -295,12 +301,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 }
 
 template <int EPI, int BN>
-static int32_t launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t s) {
+static int32_t launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t s) {
   static PerDeviceOnce once;
   const int32_t rc = set_max_smem_once(gemm_bf16_kernel<EPI, BN>, GemmTile<BN>::kSmem, once, "cudaFuncSetAttribute(gemm smem)");
   if (rc) return rc;
   const int m_tiles = (p.M + kBM - 1) / kBM, n_tiles = (p.N + BN - 1) / BN;
   const int total = m_tiles * n_tiles;
+  p.total_tiles = total;
   const int grid = total < num_sms() ? total : num_sms();
   gemm_bf16_kernel<EPI, BN><<<grid, kGemmThreads, GemmTile<BN>::kSmem, s>>>(ta, tb, p);
   MC_CHECK_LAUNCH("gemm_bf16_kernel launch");
@@ -337,7 +344,7 @@ extern "C" int32_t mc_gemm_bf16(const void* A, int64_t lda, const void* B, int64
   const int bn = mc::pick_bn(M, N);
   rc = mc::make_tmap_bf16_2d(&tb, B, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), bn, mc::kBK);
   if (rc) return rc;
-  mc::GemmParams p{M, N, K, bias, out, ldo, gate};
+  mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 #define MC_GEMM_CASE(E) \
   case E: return bn == 128 ? mc::launch_gemm_bn<E, 128>(ta, tb, p, s) : mc::launch_gemm_bn<E, 256>(ta, tb, p, s)

@@ -67,6 +67,23 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+// The same bounded wait for code that keeps wgmmas in flight across it: on timeout it sets `timed_out` and returns, and
+// once set every later wait returns at once; the caller traps after its last wgmma_wait. With a trap on the mbarrier waits
+// of attn_kernel's software-pipelined consumer loop (S(j) issued with PV(j-1)), ptxas spills the register A operand and
+// serialises every wgmma (C7512) with registers to spare; with this flag and one trap after the loop it allocates the
+// pipeline without spills.
+__device__ __forceinline__ void mbar_wait_or_flag(uint64_t* bar, uint32_t parity, bool& timed_out) {
+  if (timed_out || mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > MC_MBAR_TIMEOUT_CYCLES) {
+      MC_DIAG("mbar_wait timeout: block (%d,%d,%d) thread %d bar smem+%u parity %u\n", blockIdx.x, blockIdx.y, blockIdx.z,
+              threadIdx.x, smem_u32(bar), parity);
+      timed_out = true;
+      return;
+    }
+  }
+}
 
 // Named barriers (bar.sync / bar.arrive with an explicit id and thread count, a multiple of 32). Id 0 is __syncthreads'.
 // bar.arrive does not wait; bar.sync waits until `count` threads have arrived or synced on `id`. No timeout exists for these:
