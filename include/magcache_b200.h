@@ -150,6 +150,15 @@ int32_t mc_cfg_step(const float* cond, const float* uncond, float guide_scale, c
                     const float* const* hist, const float* coef_h, int32_t n_hist, float sigma, float* out, float* x0_out, int64_t n,
                     void* stream);
 
+/* FP8 weight dequantisation (MagCache4HunyuanVideo/README.md:76-96, `--use-fp8 --dit-weight ..._fp8.pt`): upstream's
+ * `fp8_linear_forward` [EXT hyvideo/modules/fp8_optimization.py] forms `qdata.to(bf16) * scale.to(bf16)` (fp8_activation_dequant)
+ * before every F.linear of a double / single block.
+ *   out[r, c] = bf16_rn(float(q[r, c]) * float(scale[r]))   q float8_e4m3fn [rows, cols], scale bf16 [rows], out bf16 [rows, cols]
+ * The scale is per row because one matrix may stack the rows of several Linears (the modulation table). Both conversions and the
+ * fp32 product are exact, so the result is bit-equal to upstream's; codes 0x7F / 0xFF give NaN. Contiguous operands; 16-byte loads
+ * when cols % 16 == 0 and q / out are 16-byte aligned, one element per thread otherwise. HBM-bound (3 bytes per element). */
+int32_t mc_dequant_fp8_bf16(const void* q, const void* scale, void* out, int64_t rows, int32_t cols, void* stream);
+
 /* calibration statistics                              magcache_generate.py:167-169 (one pass instead of ~7 + 3 syncs).
  * r_cur, r_prev: [rows, cols]. stats (device, 4 doubles, overwritten): sum(ratio), sum(ratio^2), sum(1-cos), rows
  * with ratio = ||r_cur[i]||2 / (||r_prev[i]||2 + denom_eps)  (denom_eps = 0 Wan :167; 1e-8 eval variant wan_magcache.py:652)

@@ -91,6 +91,7 @@ SIGNATURES = {
                     c_void_p, c_int64, c_void_p],
     "mc_residual_stats": [c_void_p, c_int32, c_void_p, c_int32, c_int64, c_int32, c_double, c_void_p, c_void_p],
     "mc_residual_sub_stats": [c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_int64, c_int32, c_double, c_void_p, c_void_p],
+    "mc_dequant_fp8_bf16": [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_void_p],
     "mc_patchify": [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p],
     "mc_ln_modulate": [c_void_p, c_int32, c_int64, c_int32, c_float, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p,
                        c_int32, c_void_p],

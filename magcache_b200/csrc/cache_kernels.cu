@@ -2,8 +2,11 @@
 //   K1 cache-hit add     `x = x + residual_x`            MagCache4Wan2.1/magcache_generate.py:295
 //   K2 residual sub      `residual_x = x - ori_x`        MagCache4Wan2.1/magcache_generate.py:299
 //   K3 calibration stats  norm ratio / std / cos distance MagCache4Wan2.1/magcache_generate.py:167-169
+//   FP8 weight dequantisation of HunyuanVideo --use-fp8 checkpoints (MagCache4HunyuanVideo/README.md:76-96)
 // Layout: flat contiguous tensors; every thread moves 128-bit words with L1::no_allocate (streamed once),
 // UNROLL independent word-groups in flight per thread, grid = a multiple of the SM count (persistent grid-stride).
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -466,9 +469,73 @@ static int32_t launch_stats(const void* cur, const void* xi, void* r_out, const 
   return MC_OK;
 }
 
+// ---- FP8 weight dequantisation: out[r, c] = bf16_rn(float(q[r, c]) * float(scale[r])) ----------------------------------------
+// float(e4m3) is exact in fp16 and fp32, and the product of a 4-bit and an 8-bit significand is exact in fp32, so the one rounding
+// is the bf16 one: bit-equal to `q.to(bf16) * scale.to(bf16)` (hyvideo fp8_activation_dequant). e4m3 0x7F / 0xFF decode to NaN.
+__device__ __forceinline__ float2 e4m3x2_to_f32x2(uint32_t pair) {  // low byte -> .x, high byte -> .y
+  uint32_t h2;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(static_cast<unsigned short>(pair & 0xFFFFu)));
+  __half2 h;
+  memcpy(&h, &h2, 4);
+  return __half22float2(h);
+}
+
+// one 16-byte word of codes (16 elements of one row) -> two 16-byte words of bf16; grid-stride over the words
+__global__ void __launch_bounds__(256) dequant_fp8_kernel(const uint8_t* __restrict__ q, const __nv_bfloat16* __restrict__ scale,
+                                                          __nv_bfloat16* __restrict__ out, int64_t n_words, int64_t words_per_row) {
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t g = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; g < n_words; g += stride) {
+    const uint4 w = ptx::ld_nc_v4(q + g * 16);
+    const float s = __bfloat162float(scale[g / words_per_row]);
+    const uint32_t wd[4] = {w.x, w.y, w.z, w.w};
+    float f[2][8];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 a = e4m3x2_to_f32x2(wd[k]), b = e4m3x2_to_f32x2(wd[k] >> 16);
+      f[k / 2][(k % 2) * 4 + 0] = __fmul_rn(a.x, s);
+      f[k / 2][(k % 2) * 4 + 1] = __fmul_rn(a.y, s);
+      f[k / 2][(k % 2) * 4 + 2] = __fmul_rn(b.x, s);
+      f[k / 2][(k % 2) * 4 + 3] = __fmul_rn(b.y, s);
+    }
+    // plain stores: the GEMM that follows reads this scratch right away, so whatever of it stays in L2 is a hit
+    uint4* o = reinterpret_cast<uint4*>(out + g * 16);
+    o[0] = pack_bf16x8(f[0]);
+    o[1] = pack_bf16x8(f[1]);
+  }
+}
+
+// any row length / alignment: one element per thread
+__global__ void __launch_bounds__(256) dequant_fp8_scalar_kernel(const uint8_t* __restrict__ q, const __nv_bfloat16* __restrict__ scale,
+                                                                 __nv_bfloat16* __restrict__ out, int64_t n, int64_t cols) {
+  const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x;
+  for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += stride)
+    out[i] = __float2bfloat16_rn(__fmul_rn(e4m3x2_to_f32x2(q[i]).x, __bfloat162float(scale[i / cols])));
+}
+
 }  // namespace mc
 
 extern "C" {
+
+int32_t mc_dequant_fp8_bf16(const void* q, const void* scale, void* out, int64_t rows, int32_t cols, void* stream) {
+  MC_CHECK_ARG(rows >= 0 && cols >= 1, "mc_dequant_fp8_bf16: rows=%lld cols=%d", static_cast<long long>(rows), cols);
+  if (rows == 0) return MC_OK;
+  MC_CHECK_ARG(q && scale && out, "mc_dequant_fp8_bf16: null pointer");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int64_t n = rows * cols;
+  const int64_t cap = static_cast<int64_t>(mc::num_sms()) * 8;  // 8 resident CTAs of 256 threads per SM
+  if (cols % 16 == 0 && mc::aligned16(q) && mc::aligned16(out)) {
+    const int64_t words = n / 16, want = (words + 255) / 256;
+    mc::dequant_fp8_kernel<<<static_cast<int>(want < cap ? want : cap), 256, 0, s>>>(
+        static_cast<const uint8_t*>(q), static_cast<const __nv_bfloat16*>(scale), static_cast<__nv_bfloat16*>(out), words, cols / 16);
+    MC_CHECK_LAUNCH("dequant_fp8_kernel launch");
+    return MC_OK;
+  }
+  const int64_t want = (n + 255) / 256;
+  mc::dequant_fp8_scalar_kernel<<<static_cast<int>(want < cap ? want : cap), 256, 0, s>>>(
+      static_cast<const uint8_t*>(q), static_cast<const __nv_bfloat16*>(scale), static_cast<__nv_bfloat16*>(out), n, cols);
+  MC_CHECK_LAUNCH("dequant_fp8_scalar_kernel launch");
+  return MC_OK;
+}
 
 int32_t mc_cache_hit_add(const void* x, int32_t x_dtype, const void* r, int32_t r_dtype, void* out, int32_t out_dtype, int64_t n,
                          void* stream) {

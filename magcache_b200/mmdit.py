@@ -40,9 +40,51 @@ def _b(t, dev):
     return t.detach().to(device=dev, dtype=torch.bfloat16).float().contiguous()  # bf16 parameter values, kept as fp32 for the epilogues
 
 
+# ----------------------------------------------------------------------------------------------------------------------
+# FP8 block weights (HunyuanVideo `--use-fp8`, MagCache4HunyuanVideo/README.md:76-96). Upstream's `convert_fp8_linear`
+# [EXT hyvideo/modules/fp8_optimization.py] stores the weight of every Linear under `double_blocks` / `single_blocks` as
+# float8_e4m3fn with a bf16 scalar `fp8_scale`; `fp8_linear_forward` multiplies by `qdata.to(bf16) * scale` in an ordinary bf16
+# F.linear. Only `Fp8Weight` and `linear()` below know that format; everything else passes weights through `linear()`.
+# ----------------------------------------------------------------------------------------------------------------------
+class Fp8Weight:
+    """float8_e4m3fn codes [rows, cols] and one bf16 scale per row (the Linear's `fp8_scale` repeated over its rows, so a row block
+    of a fused matrix and the stacked modulation rows of several Linears carry their own scales). Indexing takes a row block."""
+
+    def __init__(self, q, scale):
+        assert q.dtype == torch.float8_e4m3fn and q.dim() == 2 and scale.dtype == torch.bfloat16 and scale.shape == (q.shape[0],)
+        self.q, self.scale = q, scale
+
+    @property
+    def shape(self):
+        return self.q.shape
+
+    def __getitem__(self, rows):
+        return Fp8Weight(self.q[rows], self.scale[rows])
+
+
+def linear(a, w, bias, epilogue, out, gate=None, scratch=None):
+    """`ops.gemm(a, w, ...)` for a bf16 weight. For an Fp8Weight: per block of rows that fits `scratch` (bf16), one
+    `dequant_fp8_bf16` into the scratch, then the unchanged bf16 GEMM on it for the matching output columns. Every epilogue but
+    MC_EPI_ROWBIAS_BF16 is column-wise, so the blocks compute exactly the columns one GEMM would."""
+    if not isinstance(w, Fp8Weight):
+        return ops.gemm(a, w, bias, epilogue, out=out, gate=gate)
+    assert epilogue != E.MC_EPI_ROWBIAS_BF16 and out is not None and scratch is not None
+    rows, cols = w.shape
+    step = max(8, scratch.numel() // cols // 8 * 8)  # multiples of 8 rows keep every output column block 16-byte aligned
+    for r0 in range(0, rows, step):
+        r1 = min(rows, r0 + step)
+        b = scratch[:(r1 - r0) * cols].view(r1 - r0, cols)
+        ops.dequant_fp8_bf16(w.q[r0:r1], w.scale[r0:r1], out=b)
+        ops.gemm(a, b, None if bias is None else bias[r0:r1], epilogue, out=out[:, r0:r1], gate=None if gate is None else gate[r0:r1])
+    return out
+
+
 class FluxWeights:
     """Weights of one FluxTransformer2DModel (diffusers attribute names), repacked: q|k weights concatenated, every AdaLayerNorm
     projection stacked into one matrix, biases / norm weights as fp32 copies of their bf16 values."""
+
+    ada_parts = None    # bf16 weights only: the modulation table is one GEMM over `ada_w`
+    fp8_scratch = None
 
     def __init__(self):
         self.double, self.single = [], []
@@ -172,8 +214,18 @@ class MMDiTCore:
         """Every `Linear(silu(vec))` of the block stack (AdaLayerNormZero / ModulateDiT / final layer) from ONE GEMM: they depend on the
         conditioning vector only. bf16 like the reference, then an exact fp32 copy for the kernels that read modulation / gates."""
         w = self.w
-        ops.gemm(ops.silu(vec), w.ada_w, w.ada_b, E.MC_EPI_BIAS_BF16, out=self.ada)
+        if w.ada_parts is None:
+            ops.gemm(ops.silu(vec), w.ada_w, w.ada_b, E.MC_EPI_BIAS_BF16, out=self.ada)
+        else:  # FP8 block rows and bf16 final-layer rows: each output column still comes from its own row of the stack
+            s = ops.silu(vec)
+            for r0, wt in w.ada_parts:
+                r1 = r0 + wt.shape[0]
+                self._linear(s, wt, w.ada_b[r0:r1], E.MC_EPI_BIAS_BF16, out=self.ada[:, r0:r1])
         ops.cast_into(self.ada.view(-1), self.adaf)
+
+    def _linear(self, a, wt, bias, epilogue, out, gate=None):
+        """A block Linear: bf16 or Fp8Weight (`linear`), through the weights' dequantisation scratch."""
+        return linear(a, wt, bias, epilogue, out, gate=gate, scratch=self.w.fp8_scratch)
 
     def _rope_for(self, rows):
         """RoPE table rows for a token range, or None when that range gets no RoPE (HunyuanVideo text tokens)."""
@@ -187,7 +239,7 @@ class MMDiTCore:
             # K | V straight into the exchange's gathered buffer: image rows into this rank's segment (pushed to the peers by
             # `_joint_attention`), text rows into the local tail; q stays local
             own, tail = self._kv_views()
-            ops.gemm(h_rows, qk_w[:D], qk_b[:D], E.MC_EPI_BIAS_BF16, out=self.q_loc[rows])
+            self._linear(h_rows, qk_w[:D], qk_b[:D], E.MC_EPI_BIAS_BF16, out=self.q_loc[rows])
             if rows == self.img:
                 parts = ((h_rows, own),)
             elif rows == self.txt:
@@ -195,11 +247,11 @@ class MMDiTCore:
             else:  # the whole local sequence (single-stream blocks)
                 parts = ((h_rows[self.img], own), (h_rows[self.txt], tail))
             for hp, dst in parts:
-                ops.gemm(hp, qk_w[D:], qk_b[D:], E.MC_EPI_BIAS_BF16, out=dst[:, :D])
-                ops.gemm(hp, v_w, v_b, E.MC_EPI_BIAS_BF16, out=dst[:, D:])
+                self._linear(hp, qk_w[D:], qk_b[D:], E.MC_EPI_BIAS_BF16, out=dst[:, :D])
+                self._linear(hp, v_w, v_b, E.MC_EPI_BIAS_BF16, out=dst[:, D:])
             return
-        ops.gemm(h_rows, qk_w, qk_b, E.MC_EPI_BIAS_BF16, out=self.qk[rows])
-        ops.gemm(h_rows, v_w, v_b, E.MC_EPI_BIAS_BF16, out=self.v[rows])
+        self._linear(h_rows, qk_w, qk_b, E.MC_EPI_BIAS_BF16, out=self.qk[rows])
+        self._linear(h_rows, v_w, v_b, E.MC_EPI_BIAS_BF16, out=self.v[rows])
 
     def _qk_norm(self, rows, nq, nk):
         """Per-head RMSNorm of q and k (+ RoPE where the family applies it), in place."""
@@ -254,24 +306,24 @@ class MMDiTCore:
             self._qk_norm(img, b["nq"], b["nk"])
             self._qk_norm(txt, b["cnq"], b["cnk"])
             self._joint_attention(self.att)
-            ops.gemm(self.att[img], b["o_w"], b["o_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[img], gate=em[2])
-            ops.gemm(self.att[txt], b["co_w"], b["co_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[txt], gate=emc[2])
+            self._linear(self.att[img], b["o_w"], b["o_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[img], gate=em[2])
+            self._linear(self.att[txt], b["co_w"], b["co_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[txt], gate=emc[2])
             for rows, e, f1w, f1b, f2w, f2b in ((img, em, b["ff1_w"], b["ff1_b"], b["ff2_w"], b["ff2_b"]),
                                                 (txt, emc, b["cff1_w"], b["cff1_b"], b["cff2_w"], b["cff2_b"])):
                 ops.ln_modulate(hs[rows], e, 4, 3, round_ln_to_bf16=True, out=h[rows])
                 ffh = self.cat[rows][:, D:]
-                ops.gemm(h[rows], f1w, f1b, E.MC_EPI_BIAS_GELU_BF16, out=ffh)
-                ops.gemm(ffh, f2w, f2b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[rows], gate=e[5])
+                self._linear(h[rows], f1w, f1b, E.MC_EPI_BIAS_GELU_BF16, out=ffh)
+                self._linear(ffh, f2w, f2b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[rows], gate=e[5])
         allr = slice(0, S)
         for b in w.single:
             em = self._em(b["ada"], 3)  # (shift, scale, gate)
             ops.ln_modulate(hs, em, 1, 0, round_ln_to_bf16=True, out=h)
-            ops.gemm(h, b["mlp_w"], b["mlp_b"], E.MC_EPI_BIAS_GELU_BF16, out=self.cat[:, D:])
+            self._linear(h, b["mlp_w"], b["mlp_b"], E.MC_EPI_BIAS_GELU_BF16, out=self.cat[:, D:])
             self._project(allr, h, b["qk_w"], b["qk_b"], b["v_w"], b["v_b"])
             self._qk_norm(img, b["nq"], b["nk"])
             self._qk_norm(txt, b["nq"], b["nk"])
             self._joint_attention(self.cat[:, :D])
-            ops.gemm(self.cat, b["out_w"], b["out_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs, gate=em[2])
+            self._linear(self.cat, b["out_w"], b["out_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs, gate=em[2])
         return hs[img]
 
     def _time_mlp(self, x_bf16, mlp):
@@ -395,9 +447,44 @@ class FluxEngine(MMDiTCore):
 # ======================================================================================================================
 # HunyuanVideo
 # ======================================================================================================================
+def _fp8_blocks(m):
+    """True when `m` is an FP8 checkpoint as upstream's `convert_fp8_linear` leaves it: every Linear under `double_blocks` /
+    `single_blocks` holds float8_e4m3fn codes and an `fp8_scale`. False for a module without FP8 parameters."""
+    f8 = {name for name, p in m.named_parameters() if p.dtype == torch.float8_e4m3fn}
+    if not f8:
+        return False
+    lins = {name for name, mod in m.named_modules()
+            if name.startswith(("double_blocks.", "single_blocks.")) and isinstance(mod, torch.nn.Linear)}
+    outside = sorted(f8 - {f"{n}.weight" for n in lins})
+    if outside:
+        raise NotImplementedError(f"magcache_b200: FP8 parameters outside the block Linears are not supported: {outside[:4]}")
+    missing = sorted(n for n in lins if m.get_submodule(n).weight.dtype != torch.float8_e4m3fn)
+    if missing:
+        raise NotImplementedError(f"magcache_b200: an FP8 checkpoint must hold every block Linear in FP8; bf16: {missing[:4]}")
+    no_scale = sorted(n for n in lins if getattr(m.get_submodule(n), "fp8_scale", None) is None)
+    if no_scale:
+        raise ValueError(f"magcache_b200: FP8 weight without `fp8_scale` (upstream convert_fp8_linear sets it): {no_scale[:4]}")
+    return True
+
+
+def _fp8_scratch(w, dev):
+    """bf16 scratch for the largest FP8 weight one GEMM reads (linear2 of a single block, D x 5D: linear1 is read as its q|k, v and
+    mlp row blocks); the modulation table goes through it in row blocks."""
+    n = max(v.q.numel() for blk in w.double + w.single for v in blk.values() if isinstance(v, Fp8Weight))
+    return torch.empty(n, dtype=torch.bfloat16, device=dev)
+
+
 class HunyuanWeights:
     """Weights of one HYVideoDiffusionTransformer (hyvideo attribute names), repacked like FluxWeights: fused qkv / linear1 matrices
-    split into q|k, v (and mlp) row blocks, every ModulateDiT / final adaLN projection stacked into one matrix."""
+    split into q|k, v (and mlp) row blocks, every ModulateDiT / final adaLN projection stacked into one matrix.
+
+    An FP8 checkpoint (upstream `convert_fp8_linear`: every Linear under `double_blocks` / `single_blocks` holds float8_e4m3fn codes
+    and a bf16 `fp8_scale`) stays in FP8: the block weights become `Fp8Weight`s — row blocks of the module's own codes, 1 byte per
+    parameter, no bf16 copy — the block modulation rows are stacked as codes with a per-row scale (`ada_parts`), and one bf16
+    scratch for the largest weight a GEMM reads (`fp8_scratch`) is allocated here, once."""
+
+    ada_parts = None    # bf16 weights: the modulation table is one GEMM over `ada_w`
+    fp8_scratch = None
 
     def __init__(self):
         self.double, self.single, self.refiner = [], [], []
@@ -440,36 +527,52 @@ class HunyuanWeights:
             r_ada_w.append(blk.adaLN_modulation[1].weight.detach())
             r_ada_b.append(blk.adaLN_modulation[1].bias.detach())
         w.r_ada_w, w.r_ada_b = _w(torch.cat(r_ada_w, 0), dev), _b(torch.cat(r_ada_b, 0), dev)
-        ada_w, ada_b, off = [], [], 0
+        ada_w, ada_b, ada_lins, off = [], [], [], 0
+        fp8 = _fp8_blocks(m)
+
+        def lw(lin, rows=slice(None)):
+            """A block Linear's weight (row block `rows`): bf16, or in FP8 as views of the module's own codes."""
+            if not fp8:
+                return _w(lin.weight[rows], dev)
+            q = lin.weight.detach()[rows].to(dev)
+            return Fp8Weight(q, lin.fp8_scale.detach().to(device=dev, dtype=torch.bfloat16).reshape(1).expand(q.shape[0]).contiguous())
 
         def ada(lin):
             nonlocal off
             ada_w.append(lin.weight.detach())
             ada_b.append(lin.bias.detach())
+            ada_lins.append(lin)
             start, off = off, off + lin.weight.shape[0]
             return start
 
         for blk in m.double_blocks:
             d = {"ada": ada(blk.img_mod.linear), "ada_c": ada(blk.txt_mod.linear)}
             for pre, key in (("img", ""), ("txt", "c")):
-                W, Bq = getattr(blk, f"{pre}_attn_qkv").weight, getattr(blk, f"{pre}_attn_qkv").bias
-                proj, mlp = getattr(blk, f"{pre}_attn_proj"), getattr(blk, f"{pre}_mlp")
-                d.update({f"{key}qk_w": _w(W[:2 * D], dev), f"{key}qk_b": _b(Bq[:2 * D], dev), f"{key}v_w": _w(W[2 * D:], dev), f"{key}v_b": _b(Bq[2 * D:], dev),
+                qkv, proj, mlp = getattr(blk, f"{pre}_attn_qkv"), getattr(blk, f"{pre}_attn_proj"), getattr(blk, f"{pre}_mlp")
+                Bq = qkv.bias
+                d.update({f"{key}qk_w": lw(qkv, slice(0, 2 * D)), f"{key}qk_b": _b(Bq[:2 * D], dev), f"{key}v_w": lw(qkv, slice(2 * D, None)), f"{key}v_b": _b(Bq[2 * D:], dev),
                           f"{key}nq": _b(getattr(blk, f"{pre}_attn_q_norm").weight, dev), f"{key}nk": _b(getattr(blk, f"{pre}_attn_k_norm").weight, dev),
-                          f"{key}o_w": _w(proj.weight, dev), f"{key}o_b": _b(proj.bias, dev),
-                          f"{key}ff1_w": _w(mlp.fc1.weight, dev), f"{key}ff1_b": _b(mlp.fc1.bias, dev),
-                          f"{key}ff2_w": _w(mlp.fc2.weight, dev), f"{key}ff2_b": _b(mlp.fc2.bias, dev)})
+                          f"{key}o_w": lw(proj), f"{key}o_b": _b(proj.bias, dev),
+                          f"{key}ff1_w": lw(mlp.fc1), f"{key}ff1_b": _b(mlp.fc1.bias, dev),
+                          f"{key}ff2_w": lw(mlp.fc2), f"{key}ff2_b": _b(mlp.fc2.bias, dev)})
             w.double.append(d)
         for blk in m.single_blocks:
-            W, Bq = blk.linear1.weight, blk.linear1.bias
+            l1, Bq = blk.linear1, blk.linear1.bias
             w.single.append({
                 "ada": ada(blk.modulation.linear),
-                "qk_w": _w(W[:2 * D], dev), "qk_b": _b(Bq[:2 * D], dev), "v_w": _w(W[2 * D:3 * D], dev), "v_b": _b(Bq[2 * D:3 * D], dev),
-                "mlp_w": _w(W[3 * D:], dev), "mlp_b": _b(Bq[3 * D:], dev), "nq": _b(blk.q_norm.weight, dev), "nk": _b(blk.k_norm.weight, dev),
-                "out_w": _w(blk.linear2.weight, dev), "out_b": _b(blk.linear2.bias, dev),
+                "qk_w": lw(l1, slice(0, 2 * D)), "qk_b": _b(Bq[:2 * D], dev), "v_w": lw(l1, slice(2 * D, 3 * D)), "v_b": _b(Bq[2 * D:3 * D], dev),
+                "mlp_w": lw(l1, slice(3 * D, None)), "mlp_b": _b(Bq[3 * D:], dev), "nq": _b(blk.q_norm.weight, dev), "nk": _b(blk.k_norm.weight, dev),
+                "out_w": lw(blk.linear2), "out_b": _b(blk.linear2.bias, dev),
             })
         w.ada_out = ada(m.final_layer.adaLN_modulation[1])
-        w.ada_w, w.ada_b, w.ada_rows = _w(torch.cat(ada_w, 0), dev), _b(torch.cat(ada_b, 0), dev), off
+        w.ada_b, w.ada_rows = _b(torch.cat(ada_b, 0), dev), off
+        if not fp8:
+            w.ada_w = _w(torch.cat(ada_w, 0), dev)
+        else:  # block rows stacked as codes (+ per-row scales), the final layer's rows stay bf16
+            mods = [lw(lin) for lin in ada_lins[:-1]]
+            q = torch.cat([x.q.view(torch.uint8) for x in mods], 0).view(torch.float8_e4m3fn)
+            w.ada_parts = [(0, Fp8Weight(q, torch.cat([x.scale for x in mods], 0))), (w.ada_out, _w(ada_w[-1], dev))]
+            w.fp8_scratch = _fp8_scratch(w, dev)
         w.out_w, w.out_b = _w(m.final_layer.linear.weight, dev), _b(m.final_layer.linear.bias, dev)
         w.device = dev
         return w

@@ -305,6 +305,20 @@ def gemm(a, b, bias=None, epilogue=_lib.MC_EPI_BIAS_BF16, out=None, gate=None, t
     return out
 
 
+def dequant_fp8_bf16(q, scale, out, tag=None):
+    """out = bf16(q * scale[row]) (`mc_dequant_fp8_bf16`): q float8_e4m3fn [rows, cols], scale bf16 [rows], out bf16 [rows, cols],
+    all contiguous. Bit-equal to `q.to(bf16) * scale[:, None]`, the weight upstream's fp8_linear_forward multiplies by."""
+    _dev(q), _dev(scale), _dev(out)
+    assert q.dtype == torch.float8_e4m3fn and scale.dtype == torch.bfloat16 and out.dtype == torch.bfloat16
+    assert q.dim() == 2 and q.is_contiguous() and scale.is_contiguous() and out.is_contiguous()
+    rows, cols = q.shape
+    assert scale.shape == (rows,) and out.shape == (rows, cols)
+    with _Timed(tag, "dequant_fp8"):
+        check(lib.mc_dequant_fp8_bf16(q.data_ptr(), scale.data_ptr(), out.data_ptr(), rows, cols, _stream()))
+    _count()
+    return out
+
+
 _WORKSPACES = {}  # (kind, device index) -> torch.uint8 scratch owned by this module (grown on demand, never shrunk)
 
 
