@@ -3,14 +3,18 @@
 // (`for block in self.blocks: x = block(x, **kwargs)`, MagCache4Wan2.1/magcache_generate.py:297-298; patch_embedding :237;
 // text_embedding :257-262), with the reference's elementwise follow-ups fused into the epilogue (SURVEY §2.2 K8/K12/K13).
 //
-// Persistent kernel, one CTA per SM, tile 128 (M) x BN (N) x 64 (K per stage), BN = 256 or 128:
-//   warpgroup 0  TMA producer (one warp): A tile (128x64) + B tile (BNx64) per stage, 128-byte swizzle, 4-stage smem ring
-//   warpgroups 1-2  consumers: each owns 64 rows of the tile, wgmma m64nBNk16 x4 per stage with both operands in shared
-//                memory and the accumulator in registers; a stage goes back to the producer as soon as the wgmmas reading it
-//                have retired (one group kept in flight). Epilogue: accumulator -> per-warp 32x32 smem patch -> lane = column,
-//                so every global access is a coalesced row segment.
-// Tiles are walked in waves of gridDim.x consecutive tiles with N fastest: the CTAs of one wave share A row-panels in L2.
-// The 128-wide instantiation serves grids that would leave a wave of 256-wide tiles mostly empty (pick_bn).
+// Persistent kernel, one CTA per SM, clusters of 2 CTAs along M. A cluster walks 256 (M) x BN (N) tiles, BN = 256 or 128; at
+// each step CTA rank r of the cluster computes rows [128 r, 128 r + 128) of the tile, 64 (K) per stage:
+//   warpgroup 0  TMA producer (one warp): per stage its own A tile (128x64) and one half of the B tile (BN/2 x 64), the B half
+//                multicast into both CTAs of the cluster, so each CTA reads 16 + BN/2 * 128 bytes from L2 per stage (a third
+//                less per FLOP than loading the whole B tile) and still receives it all; 128-byte swizzle, 4-stage smem ring
+//   warpgroups 1-2  consumers: each owns 64 rows of the CTA's tile, wgmma m64nBNk16 x4 per stage with both operands in shared
+//                memory and the accumulator in registers; a stage goes back to the producers of both CTAs as soon as the wgmmas
+//                reading it have retired (one group kept in flight). Epilogue: each warp's 16 accumulator rows -> its own 16x32
+//                smem patch -> lane = column, so every global access is a coalesced row segment and all eight warps drain at
+//                the same time, with no barrier between warps.
+// Tiles are walked in waves of (number of clusters) consecutive tiles with N fastest: the CTAs of one wave share A row-panels in
+// L2. The 128-wide instantiation serves grids that would leave a wave of 256-wide tiles mostly empty (pick_bn).
 #include <cstdlib>
 
 #include "common.cuh"
@@ -28,20 +32,24 @@ std::mutex& tmap_cache_mutex() {
   return m;
 }
 
-constexpr int kBM = 128, kBK = 64, kStages = 4;
-constexpr int kTileABytes = kBM * kBK * 2;  // 16 KB
+constexpr int kCluster = 2;                    // CTAs per cluster, stacked along M
+constexpr int kBM = 128, kBK = 64, kStages = 4;  // kBM: rows of one CTA step, 64 per consumer warpgroup
+constexpr int kClusterBM = kCluster * kBM;     // rows of one cluster step (the tile the walk and pick_bn count)
+constexpr int kTileABytes = kBM * kBK * 2;     // 16 KB
 constexpr int kStagePad = 33;                                 // floats per staged row (conflict-free transpose)
 constexpr int kEpiWarps = 8;                                   // the two consumer warpgroups
-constexpr int kStagingBytes = kEpiWarps * 32 * kStagePad * 4;  // one 32x32 fp32 patch per consumer warp
+constexpr int kPatchRows = 16;                                 // a warp's rows of the accumulator fragment
+constexpr int kStagingBytes = kEpiWarps * kPatchRows * kStagePad * 4;  // one 16x32 fp32 patch per consumer warp
 constexpr int kGemmThreads = 128 + 32 * kEpiWarps;             // producer warpgroup + two consumer warpgroups
 constexpr int kProducerRegs = 40, kConsumerRegs = 232;         // setmaxnreg: 40 * 128 + 232 * 256 <= 64K
 template <int BN>
 struct GemmTile {  // BN = 256 (default) or 128
-  static constexpr int kTileBBytes = BN * kBK * 2;                 // 32 / 16 KB
-  static constexpr int kStageBytes = kTileABytes + kTileBBytes;
+  static constexpr int kTileBBytes = BN * kBK * 2;                 // 32 / 16 KB, half of it loaded by each CTA of the cluster
+  static constexpr int kHalfBBytes = kTileBBytes / kCluster;
+  static constexpr int kStageBytes = kTileABytes + kTileBBytes;    // 48 / 32 KB: what lands in each CTA per stage
   static constexpr int kOffStaging = kStages * kStageBytes;        // 196608 / 131072
-  static constexpr int kOffBars = kOffStaging + kStagingBytes;     // + 33792
-  static constexpr int kSmem = kOffBars + 128;                     // 230528 / 164992 of the 232448 an H100 block may use
+  static constexpr int kOffBars = kOffStaging + kStagingBytes;     // + 16896
+  static constexpr int kSmem = kOffBars + 128;                     // 213632 / 148096 of the 232448 an H100 block may use
 };
 
 struct GemmParams {
@@ -50,14 +58,14 @@ struct GemmParams {
   void* out;
   int64_t ldo;
   const float* gate;
-  int total_tiles;  // m tiles x n tiles, set by launch_gemm_bn: read from the parameter bank, the loop bound costs no register
+  int total_tiles;  // 256-row m tiles x n tiles (cluster steps), set by launch_gemm_bn: read from the parameter bank
 };
 
-// One 32-row x 32-column patch: `stage` holds acc[r][c] at stage[r*33 + c]; lane = column. All global accesses below
+// One ROWS-row x 32-column patch: `stage` holds acc[r][c] at stage[r*33 + c]; lane = column. All global accesses below
 // touch 128 (fp32) or 64 (bf16, two rows per instruction) contiguous bytes per row.
-template <int EPI>
+template <int EPI, int ROWS>
 __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float* stage, int row0, int col0, int lane) {
-  const int rows = min(32, p.M - row0);
+  const int rows = min(ROWS, p.M - row0);
   if (rows <= 0) return;
   const int col = col0 + lane;
   const bool col_ok = col < p.N;
@@ -67,10 +75,9 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
     const float b = (p.bias && col_ok) ? p.bias[col] : 0.f;
     const float g = (p.gate && col_ok) ? p.gate[col] : 1.f;
     float* xcol = static_cast<float*>(p.out) + static_cast<int64_t>(row0) * p.ldo + col;
-    // two halves of 16 rows, 16 loads in flight each: all 32 rows at once spilled next to the 256-wide tile's 128 accumulator
-    // registers (same operations per element, same order)
+    // 16 rows at a time, 16 loads in flight: all 32 rows at once spilled next to the 256-wide tile's 128 accumulator registers
 #pragma unroll
-    for (int h = 0; h < 32; h += 16) {
+    for (int h = 0; h < ROWS; h += 16) {
       float xv[16];
 #pragma unroll
       for (int r = 0; r < 16; ++r) xv[r] = (col_ok && h + r < rows) ? xcol[static_cast<int64_t>(h + r) * p.ldo] : 0.f;
@@ -90,7 +97,7 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
     const float b = (p.bias && col_ok) ? p.bias[col] : 0.f;
     float* ocol = static_cast<float*>(p.out) + static_cast<int64_t>(row0) * p.ldo + col;
 #pragma unroll
-    for (int r = 0; r < 32; ++r)
+    for (int r = 0; r < ROWS; ++r)
       if (col_ok && r < rows) ocol[static_cast<int64_t>(r) * p.ldo] = stage[r * kStagePad + lane] + b;
     return;
   }
@@ -112,11 +119,11 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
   const float* sbase = stage + half * kStagePad + cp;
   const float* rbias = (EPI == MC_EPI_ROWBIAS_BF16 && p.bias) ? p.bias + row0 + half : nullptr;
 
-  if (rows == 32 && col0 + 32 <= p.N && (p.ldo & 1) == 0) {
-    // interior patch: branch-free, 16 independent iterations for the scheduler to interleave
-    uint32_t w[16];
+  if (rows == ROWS && col0 + 32 <= p.N && (p.ldo & 1) == 0) {
+    // interior patch: branch-free, ROWS / 2 independent iterations for the scheduler to interleave
+    uint32_t w[ROWS / 2];
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
+    for (int i = 0; i < ROWS / 2; ++i) {
       float v0 = sbase[2 * i * kStagePad], v1 = sbase[2 * i * kStagePad + 1];
       if (EPI == MC_EPI_ROWBIAS_BF16) {
         const float rb = rbias ? rbias[2 * i] : 0.f;  // V^T = Wv h^T + bv: bias indexed by the output ROW
@@ -146,12 +153,12 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
       w[i] = pack_bf16x2(v0, v1);
     }
 #pragma unroll
-    for (int i = 0; i < 16; ++i) *reinterpret_cast<uint32_t*>(obase + static_cast<int64_t>(2 * i) * p.ldo) = w[i];
+    for (int i = 0; i < ROWS / 2; ++i) *reinterpret_cast<uint32_t*>(obase + static_cast<int64_t>(2 * i) * p.ldo) = w[i];
     return;
   }
 
   const bool pair_ok = (c0 + 1 < p.N) && ((p.ldo & 1) == 0);
-  for (int i = 0; i < 16; ++i) {
+  for (int i = 0; i < ROWS / 2; ++i) {
     const int r = 2 * i + half;
     if (r >= rows) continue;
     float v0 = sbase[2 * i * kStagePad], v1 = sbase[2 * i * kStagePad + 1];
@@ -190,7 +197,7 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
 }
 
 template <int EPI, int kBN>
-__global__ void __launch_bounds__(kGemmThreads, 1)
+__global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kGemmThreads, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
   using T = GemmTile<kBN>;
   constexpr int kStageBytes = T::kStageBytes, kOffStaging = T::kOffStaging, kOffBars = T::kOffBars;
@@ -201,8 +208,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = (p.N + kBN - 1) / kBN;
-  const int total_tiles = p.total_tiles;
   const int num_kb = (p.K + kBK - 1) / kBK;
+  // Both CTAs of a cluster walk the same cluster tiles in lock step (the launch makes the grid at most one cluster per tile, so
+  // every cluster has at least one step); rank r takes rows [64 r, 64 r + 64) of each, computing on TMA's zero fill where
+  // those rows lie past M (the epilogue then writes nothing).
+  const uint32_t rank = ptx::cluster_ctarank();
+  const int cluster = static_cast<int>(ptx::cluster_id_x()), n_clusters = static_cast<int>(ptx::num_clusters_x());
+  const int steps = (p.total_tiles - cluster + n_clusters - 1) / n_clusters;
 
   if (threadIdx.x == 0) {
     if ((ptx::smem_u32(smem) & 1023u) != 0) {
@@ -213,28 +225,33 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
     ptx::prefetch_tmap(&tmap_b);
     for (int s = 0; s < kStages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], kEpiWarps);  // one arrival per consumer warp
+      ptx::mbar_init(&empty_bar[s], kCluster * kEpiWarps);  // one arrival per consumer warp, in each CTA
     }
     ptx::fence_mbar_init();
   }
-  __syncthreads();
+  // the peer multicasts into this CTA's ring and arrives on its empty barriers: both CTAs' barriers must be initialised first
+  ptx::cluster_arrive();
+  ptx::cluster_wait();
 
   if (warp < 4) {
     ptx::setmaxnreg_dec<kProducerRegs>();
     if (warp == 0) {
       // TMA producer: the whole warp walks the loop in uniform control flow, one elected lane issues the copies (ptx::elect_one)
-      uint32_t it = 0;  // running k-block counter across tiles -> smem stage / phase
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int m0 = (tile / n_tiles) * kBM, n0 = (tile % n_tiles) * kBN;
+      uint32_t it = 0;  // running k-block counter across steps -> smem stage / phase (the same sequence in both CTAs)
+      for (int i = 0; i < steps; ++i) {
+        const int tile = cluster + i * n_clusters;
+        const int m0 = (tile / n_tiles) * kClusterBM + static_cast<int>(rank) * kBM, n0 = (tile % n_tiles) * kBN;
+        const int nb = n0 + static_cast<int>(rank) * (kBN / kCluster);  // this CTA's half of the B tile
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const int s = it % kStages;
           const uint32_t ph = (it / kStages) & 1;
-          ptx::mbar_wait(&empty_bar[s], ph ^ 1);
+          ptx::mbar_wait(&empty_bar[s], ph ^ 1);  // released by the consumers of both CTAs: the multicast writes into both
           if (ptx::elect_one()) {
             uint8_t* sa = smem + s * kStageBytes;
-            ptx::mbar_expect_tx(&full_bar[s], kStageBytes);
+            ptx::mbar_expect_tx(&full_bar[s], kStageBytes);  // own A + both B halves
             ptx::tma_load_2d(sa, &tmap_a, &full_bar[s], kb * kBK, m0);
-            ptx::tma_load_2d(sa + kTileABytes, &tmap_b, &full_bar[s], kb * kBK, n0);
+            ptx::tma_load_2d_multicast(sa + kTileABytes + rank * T::kHalfBBytes, &tmap_b, &full_bar[s], kb * kBK, nb,
+                                       static_cast<uint16_t>((1u << kCluster) - 1));
           }
           __syncwarp();
         }
@@ -242,17 +259,21 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
     }
   } else {
     ptx::setmaxnreg_inc<kConsumerRegs>();
-    const int wg = (warp >> 2) - 1;  // consumer warpgroup: rows [64 wg, 64 wg + 64) of the tile
+    const int wg = (warp >> 2) - 1;  // consumer warpgroup: rows [64 wg, 64 wg + 64) of the CTA's tile
     const int wq = warp & 3;         // warp inside the warpgroup
     float acc[kBN / 2];
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int m0 = (tile / n_tiles) * kBM, n0 = (tile % n_tiles) * kBN;
+    // The mbarrier waits record a timeout instead of trapping (ptx::mbar_wait_or_flag: a trap on a wait inside a loop that
+    // keeps wgmmas in flight makes ptxas spill and serialise them); the trap comes after the last wgmma_wait.
+    bool timed_out = false;
+    for (int i = 0; i < steps; ++i) {
+      const int tile = cluster + i * n_clusters;
+      const int m0 = (tile / n_tiles) * kClusterBM + static_cast<int>(rank) * kBM, n0 = (tile % n_tiles) * kBN;
+      uint32_t it = static_cast<uint32_t>(i) * num_kb;
       int prev_s = -1;
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
         const int s = it % kStages;
         const uint32_t ph = (it / kStages) & 1;
-        ptx::mbar_wait(&full_bar[s], ph);
+        ptx::mbar_wait_or_flag(&full_bar[s], ph, timed_out);
         const uint32_t sa = ptx::smem_u32(smem + s * kStageBytes);
         const uint64_t da = ptx::gmma_desc_sw128_kmajor(sa + wg * (64 * 128));  // this warpgroup's 64 rows: 8 row groups of 1024 B
         const uint64_t db = ptx::gmma_desc_sw128_kmajor(sa + kTileABytes);
@@ -266,24 +287,26 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
           }
         }
         ptx::wgmma_commit();
-        ptx::wgmma_wait<1>();  // the previous stage's wgmmas have retired: hand that stage back
+        ptx::wgmma_wait<1>();  // the previous stage's wgmmas have retired: hand that stage back to both producers
         ptx::fence_regs(acc);
-        if (prev_s >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev_s]);
+        if (prev_s >= 0 && lane == 0)
+          for (uint32_t c = 0; c < kCluster; ++c) ptx::mbar_arrive_cluster(&empty_bar[prev_s], c);
         prev_s = s;
       }
       ptx::wgmma_wait<0>();
       ptx::fence_regs(acc);
-      if (lane == 0) ptx::mbar_arrive(&empty_bar[prev_s]);
+      if (lane == 0)
+        for (uint32_t c = 0; c < kCluster; ++c) ptx::mbar_arrive_cluster(&empty_bar[prev_s], c);
 
-      // epilogue, 32 columns at a time. The warp pair holding rows [32 pr, 32 pr + 32) of this warpgroup (16 rows each) fills
-      // one 32x32 patch together; the pair has two patch buffers and alternates which warp drains them.
-      const int pr = wq >> 1;
-      const int row0 = m0 + wg * 64 + pr * 32;
-      const int r_lo = (wq & 1) * 16 + (lane >> 2);  // this warp's first row inside the patch (the second is r_lo + 8)
+      // epilogue, 32 columns at a time. Each warp stages its own 16 rows of the fragment in its own 16x32 patch and drains it,
+      // so the four warps of the warpgroup write (and, for the residual stream, load) global memory at the same time, with no
+      // barrier between warps.
+      float* patch = staging + (4 * wg + wq) * kPatchRows * kStagePad;
+      const int row0 = m0 + wg * 64 + wq * kPatchRows;
+      const int r_lo = lane >> 2;  // this lane's first row inside the patch (the second is r_lo + 8)
 #pragma unroll  // static accumulator indices: the accumulator must stay in registers
       for (int c = 0; c < kBN / 32; ++c) {
-        float* patch = staging + (4 * wg + 2 * pr + (c & 1)) * 32 * kStagePad;
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + 2 * wg + pr) : "memory");  // the patch buffer's previous reader is done
+        __syncwarp();  // the previous patch has been read
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const int i = 4 * c + q;
@@ -293,22 +316,56 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
           patch[(r_lo + 8) * kStagePad + col] = acc[4 * i + 2];
           patch[(r_lo + 8) * kStagePad + col + 1] = acc[4 * i + 3];
         }
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + 2 * wg + pr) : "memory");
-        if ((wq & 1) == (c & 1)) epilogue_patch<EPI>(p, patch, row0, n0 + c * 32, lane);
+        __syncwarp();
+        epilogue_patch<EPI, kPatchRows>(p, patch, row0, n0 + c * 32, lane);
       }
     }
+    if (timed_out) __trap();
   }
+  // no CTA may exit while its peer can still multicast into its ring or arrive on its empty barriers
+  ptx::cluster_arrive();
+  ptx::cluster_wait();
+}
+
+// Clusters of this instantiation that fit on the device at once (1 CTA per SM at this shared-memory size), cached per device.
+// Clusters live inside a GPC, so this can be less than SMs / 2; a grid of SMs / 2 clusters would then run a second, nearly
+// empty wave.
+template <int EPI, int BN>
+static int32_t max_active_clusters(int* out) {
+  static int cached[kMaxDevices] = {};
+  const int d = current_device();
+  if (cached[d] > 0) {
+    *out = cached[d];
+    return MC_OK;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(kCluster * num_sms(), 1, 1);
+  cfg.blockDim = dim3(kGemmThreads, 1, 1);
+  cfg.dynamicSmemBytes = GemmTile<BN>::kSmem;
+  int n = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, gemm_bf16_kernel<EPI, BN>, &cfg);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaOccupancyMaxActiveClusters(gemm)");
+  if (n < 1) {
+    set_error("gemm_bf16_kernel: no cluster of %d CTAs with %d B of shared memory fits on this device", kCluster, GemmTile<BN>::kSmem);
+    return MC_ERR_CUDA;
+  }
+  cached[d] = n;
+  *out = n;
+  return MC_OK;
 }
 
 template <int EPI, int BN>
 static int32_t launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t s) {
   static PerDeviceOnce once;
-  const int32_t rc = set_max_smem_once(gemm_bf16_kernel<EPI, BN>, GemmTile<BN>::kSmem, once, "cudaFuncSetAttribute(gemm smem)");
+  int32_t rc = set_max_smem_once(gemm_bf16_kernel<EPI, BN>, GemmTile<BN>::kSmem, once, "cudaFuncSetAttribute(gemm smem)");
   if (rc) return rc;
-  const int m_tiles = (p.M + kBM - 1) / kBM, n_tiles = (p.N + BN - 1) / BN;
+  int clusters = 0;
+  rc = max_active_clusters<EPI, BN>(&clusters);
+  if (rc) return rc;
+  const int m_tiles = (p.M + kClusterBM - 1) / kClusterBM, n_tiles = (p.N + BN - 1) / BN;
   const int total = m_tiles * n_tiles;
   p.total_tiles = total;
-  const int grid = total < num_sms() ? total : num_sms();
+  const int grid = kCluster * (total < clusters ? total : clusters);
   gemm_bf16_kernel<EPI, BN><<<grid, kGemmThreads, GemmTile<BN>::kSmem, s>>>(ta, tb, p);
   MC_CHECK_LAUNCH("gemm_bf16_kernel launch");
   return MC_OK;
@@ -323,7 +380,7 @@ static int pick_bn(int M, int N) {
     const int v = atoi(e);
     if (v == 128 || v == 256) return v;
   }
-  const int64_t sms = num_sms(), m_tiles = (M + kBM - 1) / kBM;
+  const int64_t sms = num_sms(), m_tiles = (M + 127) / 128;  // waves of SMs 128-row CTA steps
   const int64_t t256 = m_tiles * ((N + 255) / 256), t128 = m_tiles * ((N + 127) / 128);
   const int64_t cost256 = ((t256 + sms - 1) / sms) * 100, cost128 = ((t128 + sms - 1) / sms) * 62;
   return cost128 * 100 <= cost256 * 92 ? 128 : 256;
@@ -342,7 +399,9 @@ extern "C" int32_t mc_gemm_bf16(const void* A, int64_t lda, const void* B, int64
   int32_t rc = mc::make_tmap_bf16_2d(&ta, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(lda), mc::kBM, mc::kBK);
   if (rc) return rc;
   const int bn = mc::pick_bn(M, N);
-  rc = mc::make_tmap_bf16_2d(&tb, B, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), bn, mc::kBK);
+  // each CTA of a cluster loads (and multicasts) one half of the B tile: the box is bn / 2 rows
+  rc = mc::make_tmap_bf16_2d(&tb, B, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), bn / mc::kCluster,
+                             mc::kBK);
   if (rc) return rc;
   mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0};
   cudaStream_t s = static_cast<cudaStream_t>(stream);

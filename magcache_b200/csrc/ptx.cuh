@@ -95,6 +95,42 @@ __device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
+// ------------------------------------------------------------------------------------------------
+// thread-block clusters
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_id_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t num_clusters_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
+  return r;
+}
+// Arrive on the mbarrier at `bar`'s offset in the shared memory of cluster rank `cta` (this CTA's own rank included). Used to
+// hand a ring stage back after the wgmmas that read it have retired (wgmma.wait_group). The default .release.cta semantics
+// suffice for that and compile to a plain remote arrive; .release.cluster adds a MEMBAR.GPU before every arrival, which waits
+// for the thread's outstanding global stores (the previous tile's epilogue).
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n"
+      ".reg .b32 ra;\n"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
+      "}\n"
+      ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
+}
+// Cluster-wide barrier: every thread of every CTA of the cluster arrives, then waits for all of them.
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+
 // One lane of a fully converged warp, for the single-thread TMA issue: elected from warp-uniform control flow, the copy
 // instructions take uniform operands without a uniformisation loop around them.
 __device__ __forceinline__ bool elect_one() {
@@ -127,6 +163,16 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, ui
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+
+// The same load written into every CTA of the cluster named in `cta_mask` (bit r = cluster rank r), at the same shared-memory
+// offset in each; each destination's mbarrier at `bar`'s offset receives the complete_tx for the bytes that landed there.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0, int32_t c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 

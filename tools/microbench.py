@@ -87,23 +87,32 @@ if which in ("all", "rows"):
     rec("head_unpatchify_fused_hit", *timeit(lambda: ops.head_unpatchify(x0, hm, ee, Wt, b, (21, 30, 52), residual=xs)), bytes_=n * 6)
 
 if which in ("all", "gemm"):
-    a = torch.randn(N_TOK, D, device=dev).bfloat16()
-    for name, N, K, epi in [("gemm_qkv_1536x1536", D, D, _lib.MC_EPI_BIAS_BF16), ("gemm_ffn1_8960x1536_gelu", FFN, D, _lib.MC_EPI_BIAS_GELU_BF16)]:
+    # the block GEMMs of one Wan2.1-1.3B layer (wan.py tags), each with the epilogue the engine runs it with, next to
+    # torch.matmul (cuBLAS, plain bf16 output) on the same operands; a rate is only worth something with the card it ran on
+    import subprocess
+    try:
+        card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+    except Exception as ex:  # noqa: BLE001
+        card = f"{torch.cuda.get_device_name()} (nvidia-smi unavailable: {ex})"
+    res["card"] = card
+    print("card:", card, flush=True)
+    E = _lib
+    for tag, N, K, epi in [("gemm_qkv", 3 * D, D, E.MC_EPI_BIAS_BF16), ("gemm_o", D, D, E.MC_EPI_BIAS_GATE_RESID),
+                           ("gemm_cq", D, D, E.MC_EPI_BIAS_BF16), ("gemm_co", D, D, E.MC_EPI_BIAS_GATE_RESID),
+                           ("gemm_ffn1", FFN, D, E.MC_EPI_BIAS_GELU_BF16), ("gemm_ffn2", D, FFN, E.MC_EPI_BIAS_GATE_RESID)]:
+        a = torch.randn(N_TOK, K, device=dev).bfloat16()
         b = (torch.randn(N, K, device=dev) / math.sqrt(K)).bfloat16()
-        bias = torch.zeros(N, device=dev)
-        o = torch.empty(N_TOK, N, dtype=torch.bfloat16, device=dev)
-        rec(name, *timeit(lambda: ops.gemm(a, b, bias, epi, out=o)), flops=2.0 * N_TOK * N * K)
-        rec(name + "_cublas", *timeit(lambda: torch.matmul(a, b.t())), flops=2.0 * N_TOK * N * K)
-    wo = (torch.randn(D, D, device=dev) / math.sqrt(D)).bfloat16()
-    xs0 = torch.randn(N_TOK, D, device=dev)
-    g0 = torch.randn(D, device=dev)
-    rec("gemm_oproj_1536x1536_gate_resid", *timeit(lambda: ops.gemm(a, wo, g0, _lib.MC_EPI_BIAS_GATE_RESID, out=xs0, gate=g0)), flops=2.0 * N_TOK * D * D)
-    a2 = torch.randn(N_TOK, FFN, device=dev).bfloat16()
-    b2 = (torch.randn(D, FFN, device=dev) / math.sqrt(FFN)).bfloat16()
-    xs = torch.randn(N_TOK, D, device=dev)
-    g = torch.randn(D, device=dev)
-    rec("gemm_ffn2_1536x8960_gate_resid", *timeit(lambda: ops.gemm(a2, b2, g, _lib.MC_EPI_BIAS_GATE_RESID, out=xs, gate=g)), flops=2.0 * N_TOK * D * FFN)
-    rec("gemm_ffn2_cublas", *timeit(lambda: torch.matmul(a2, b2.t())), flops=2.0 * N_TOK * D * FFN)
+        bias = torch.randn(N, device=dev) * 0.01
+        gate = torch.randn(N, device=dev) * 0.01 if tag in ("gemm_o", "gemm_ffn2") else None
+        if epi == E.MC_EPI_BIAS_GATE_RESID:  # fp32 residual stream, updated in place
+            o = torch.randn(N_TOK, N, device=dev)
+        else:
+            o = torch.empty(N_TOK, N, dtype=torch.bfloat16, device=dev)
+        flops = 2.0 * N_TOK * N * K
+        rec(f"{tag}_{N_TOK}x{N}x{K}", *timeit(lambda: ops.gemm(a, b, bias, epi, out=o, gate=gate)), flops=flops)
+        rec(f"{tag}_cublas", *timeit(lambda: torch.matmul(a, b.t())), flops=flops)
+        del a, b, o
 
 if which in ("all", "attn"):
     q = torch.randn(N_TOK, D, device=dev).bfloat16()
