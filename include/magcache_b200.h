@@ -213,6 +213,10 @@ int32_t mc_patchify(const float* latent, int32_t C, int32_t F, int32_t H, int32_
  *   mode 0: a = 1 + p0[scale_idx], b = p0[shift_idx]   p0 = e = modulation + e0, fp32 [k, cols]  (block norm1/norm2:
  *           `norm1(x).float() * (1 + e[1]) + e[0]`, upstream WanAttentionBlock.forward); p1 unused
  *   mode 1: a = p0, b = p1                             (norm3, elementwise affine weight / bias)
+ *   mode 2: y = bf16(bf16(bf16(LN(x)) * bf16(1 + p0[scale_idx])) + p0[shift_idx])   p0 fp32 [k, cols] holding bf16 values; p1 and
+ *           round_ln_to_bf16 unused. `t2i_modulate(self.norm1(x), shift, scale)` of STDiT3Block.forward
+ *           (videosys/models/transformers/open_sora_transformer_3d.py:187, :248) and of T2IFinalLayer (:80), where every step is a
+ *           bf16 tensor op. x and out bf16, 16-byte aligned, cols <= 2048.
  * x: [rows, cols] (fp32 or bf16); round_ln_to_bf16 != 0 reproduces `.type_as(x)` for a bf16 stream (block 0).
  * out: [rows, cols] bf16 (GEMM operand) or fp32. x/out 32-byte aligned, cols % 8 == 0, cols <= 8192. */
 int32_t mc_ln_modulate(const void* x, int32_t x_dtype, int64_t rows, int32_t cols, float eps, int32_t mode,
@@ -235,6 +239,28 @@ int32_t mc_rmsnorm_rope_segs(void* x_bf16, int64_t ld, int64_t rows, int32_t seg
  * cos_sin: fp32 [rows, 128] interleaved (cos, sin) per pair, or NULL. */
 int32_t mc_rmsnorm_head_rope(void* x_bf16, int64_t ld, int64_t rows, int32_t heads, const float* w, float eps, const float* cos_sin,
                              void* stream);
+/* Open-Sora 1.2 (STDiT3, head_dim 72; csrc/opensora_kernels.cu) ------------------------------------------------------------
+ * q / k normalisation of OpenSoraAttention.forward (videosys/models/modules/attentions.py:71-75, `qk_norm_legacy=False`): per-head
+ * LlamaRMSNorm(72) (normalization.py:17-22: y = bf16(w * bf16(x * rsqrt(mean x^2 + eps))), w fp32 copies of the bf16 weight [72]),
+ * then, when cos_sin != NULL, RoPE on interleaved pairs in fp32 rounded to bf16 (rotary_embedding_torch
+ * `RotaryEmbedding(72).rotate_queries_or_keys` [EXT]), in place on x bf16 [rows, heads*72] (row pitch ld % 8 == 0).
+ * cos_sin: fp32 [pos_mod, 72] = (cos, sin) per pair; row r uses position (r / pos_div) % pos_mod — the frame index of a B (T S) C
+ * token row with pos_div = S, pos_mod = T. */
+int32_t mc_rmsnorm_head72_rope(void* x_bf16, int64_t ld, int64_t rows, int32_t heads, const float* w, float eps, const float* cos_sin,
+                               int64_t pos_div, int32_t pos_mod, void* stream);
+/* softmax(q k^T * scale) v, head_dim 72, over independent segments in one launch: segs_dev (device) int32 [n_segs, 4] =
+ * (q_start, q_len, k_start, k_len); the q rows [q_start, q_start+q_len) attend to the k / v rows [k_start, k_start+k_len) (k_len >= 1).
+ * The spatial self-attention (B*T frames of S tokens, `rearrange(x, "B (T S) C -> (B T) S C")` + OpenSoraAttention,
+ * open_sora_transformer_3d.py:202-204) and the cross-attention with per-sample caption lengths (`flash_attn_varlen_func` of
+ * OpenSoraMultiHeadCrossAttention.flash_attn_impl, attentions.py:136-153). max_q_len >= every q_len. Row-major bf16 views,
+ * leading dimensions % 8 == 0, 16-byte aligned pointers. */
+int32_t mc_attn_varlen_d72(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
+                           int32_t heads, const int32_t* segs_dev, int32_t n_segs, int32_t max_q_len, float scale, void* stream);
+/* The temporal self-attention of STDiT3Block (open_sora_transformer_3d.py:196-198) without the `rearrange` copies: the rows of
+ * q / k / v / out are in B (T S) C order, and sequence (b, s) is the T rows b*T*S + t*S + s, t < T <= 32. head_dim 72. */
+int32_t mc_attn_temporal_d72(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
+                             int32_t B, int32_t T, int32_t S, int32_t heads, float scale, void* stream);
+
 /* out[c] = bf16(bf16(sum_r x[r, c]) / rows): the mean over the valid text tokens that conditions HunyuanVideo's token refiner
  * [EXT hyvideo SingleTokenRefiner.forward, called at MagCache4HunyuanVideo/magcache_sample_video.py:69]. x bf16 [rows, cols] (row stride ld). */
 int32_t mc_colmean_bf16(const void* x, int64_t ld, int32_t rows, int32_t cols, void* out, void* stream);

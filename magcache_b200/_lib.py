@@ -98,6 +98,11 @@ SIGNATURES = {
     "mc_rmsnorm_rope": [c_void_p, c_int64, c_int64, c_int32, c_void_p, c_float, c_void_p, c_int32, c_void_p],
     "mc_rmsnorm_rope_segs": [c_void_p, c_int64, c_int64, c_int32, c_int32, c_void_p, c_float, c_void_p, c_int32, c_void_p],
     "mc_rmsnorm_head_rope": [c_void_p, c_int64, c_int64, c_int32, c_void_p, c_float, c_void_p, c_void_p],
+    "mc_rmsnorm_head72_rope": [c_void_p, c_int64, c_int64, c_int32, c_void_p, c_float, c_void_p, c_int64, c_int32, c_void_p],
+    "mc_attn_varlen_d72": [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int32, c_void_p, c_int32, c_int32,
+                           c_float, c_void_p],
+    "mc_attn_temporal_d72": [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32,
+                             c_float, c_void_p],
     "mc_colmean_bf16": [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p],
     "mc_silu_bf16": [c_void_p, c_void_p, c_int64, c_void_p],
     "mc_gemm_bf16": [c_void_p, c_int64, c_void_p, c_int64, c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_int64, c_void_p,

@@ -108,6 +108,59 @@ __global__ void __launch_bounds__(256) ln_modulate_kernel(const void* __restrict
   }
 }
 
+// ---- mode 2: LayerNorm + t2i_modulate with every step a bf16 tensor op (STDiT3Block.forward, open_sora_transformer_3d.py:187, :248;
+// T2IFinalLayer, :80): y = bf16(bf16(bf16(LN(x)) * bf16(1 + p0[scale_idx])) + p0[shift_idx]), p0 holding bf16 values.
+// One warp per row, x and out bf16, cols <= 2048.
+__global__ void __launch_bounds__(256) ln_t2i_modulate_kernel(const __nv_bfloat16* __restrict__ x, int64_t rows, int cols, float eps,
+                                                              const float* __restrict__ sc, const float* __restrict__ sh,
+                                                              __nv_bfloat16* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int groups = cols >> 3;
+  const float inv_n = 1.0f / static_cast<float>(cols);
+  for (int64_t row = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; row < rows;
+       row += (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5) {
+    float v[kMaxG][8];
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < kMaxG; ++i) {
+      const int g = lane + i * 32;
+      if (g < groups) {
+        unpack_bf16x8(ptx::ld_nc_v4(x + row * cols + g * 8), v[i]);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) s += v[i][j];
+      }
+    }
+    const float mean = warp_sum(s) * inv_n;
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < kMaxG; ++i) {
+      if (lane + i * 32 < groups) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float d = v[i][j] - mean;
+          q = fmaf(d, d, q);
+        }
+      }
+    }
+    const float rstd = rsqrtf(warp_sum(q) * inv_n + eps);
+#pragma unroll
+    for (int i = 0; i < kMaxG; ++i) {
+      const int g = lane + i * 32;
+      if (g < groups) {
+        float a[8], b[8], o[8];
+        load_param8(sc + g * 8, a);
+        load_param8(sh + g * 8, b);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float y = round_bf16((v[i][j] - mean) * rstd);
+          o[j] = round_bf16(__fadd_rn(round_bf16(__fmul_rn(y, round_bf16(__fadd_rn(1.0f, a[j])))), b[j]));
+        }
+        ptx::st_na_v4(out + row * cols + g * 8, pack_bf16x8(o));
+      }
+    }
+  }
+}
+
 // ---- WanRMSNorm over the model dim (+ optional 3-axis RoPE), in place on bf16 ---------------------------------
 template <int TPR>
 __global__ void __launch_bounds__(256) rmsnorm_rope_kernel(__nv_bfloat16* __restrict__ x, int64_t ld, int64_t rows, int cols,
@@ -756,8 +809,19 @@ int32_t mc_patchify(const float* latent, int32_t C, int32_t F, int32_t H, int32_
 int32_t mc_ln_modulate(const void* x, int32_t x_dtype, int64_t rows, int32_t cols, float eps, int32_t mode, const float* p0,
                        const float* p1, int32_t scale_idx, int32_t shift_idx, int32_t round_ln_to_bf16, void* out,
                        int32_t out_dtype, void* stream) {
-  MC_CHECK_ARG(x && p0 && out && (mode == 0 || p1), "mc_ln_modulate: null pointer");
-  MC_CHECK_ARG(mode == 0 || mode == 1, "mc_ln_modulate: bad mode %d", mode);
+  MC_CHECK_ARG(x && p0 && out && (mode != 1 || p1), "mc_ln_modulate: null pointer");
+  MC_CHECK_ARG(mode == 0 || mode == 1 || mode == 2, "mc_ln_modulate: bad mode %d", mode);
+  if (mode == 2) {
+    MC_CHECK_ARG(x_dtype == MC_BF16 && out_dtype == MC_BF16 && cols >= 8 && cols % 8 == 0 && cols <= 32 * 8 * mc::kMaxG && rows >= 1,
+                 "mc_ln_modulate: mode 2 needs bf16 x / out and cols %% 8 == 0, cols <= 2048 (cols=%d)", cols);
+    MC_CHECK_ARG(mc::aligned16(x) && mc::aligned16(out) && mc::aligned16(p0) && cols % 4 == 0, "mc_ln_modulate: mode 2 pointers must be 16-byte aligned");
+    const int64_t want = (rows + 7) / 8, cap = static_cast<int64_t>(mc::num_sms()) * 16;
+    mc::ln_t2i_modulate_kernel<<<static_cast<int>(want < cap ? want : cap), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(x), rows, cols, eps, p0 + static_cast<int64_t>(scale_idx) * cols,
+        p0 + static_cast<int64_t>(shift_idx) * cols, static_cast<__nv_bfloat16*>(out));
+    MC_CHECK_LAUNCH("ln_t2i_modulate_kernel launch");
+    return MC_OK;
+  }
   MC_CHECK_ARG(rows >= 1 && cols >= 8 && cols % 8 == 0 && cols <= 128 * 8 * mc::kMaxG, "mc_ln_modulate: cols=%d unsupported", cols);
   MC_CHECK_ARG(mc::aligned16(p0) && (p1 == nullptr || mc::aligned16(p1)), "mc_ln_modulate: parameters must be 16-byte aligned");
   MC_CHECK_ARG((x_dtype == MC_F32 || x_dtype == MC_BF16) && (out_dtype == MC_F32 || out_dtype == MC_BF16), "mc_ln_modulate: bad dtype");

@@ -263,6 +263,76 @@ def rmsnorm_head_rope_(x, weight, heads, cos_sin=None, eps=1e-6, tag=None):
     return x
 
 
+def rmsnorm_head72_rope_(x, weight, heads, cos_sin=None, pos_div=1, eps=1e-6, tag=None):
+    """In-place per-head LlamaRMSNorm(72) + optional RoPE (`mc_rmsnorm_head72_rope`) on a bf16 [rows, heads*72] view (row stride
+    allowed): the q / k normalisation of Open-Sora's attention. weight fp32 [72]; cos_sin fp32 [P, 72] (interleaved cos, sin per pair),
+    row r uses position (r // pos_div) % P."""
+    _dev(x)
+    assert x.dtype == torch.bfloat16 and x.dim() == 2 and x.stride(1) == 1 and x.shape[1] == heads * 72
+    assert weight.dtype == torch.float32 and weight.numel() == 72 and weight.is_contiguous()
+    P = 1
+    if cos_sin is not None:
+        assert cos_sin.dtype == torch.float32 and cos_sin.is_contiguous() and cos_sin.dim() == 2 and cos_sin.shape[1] == 72
+        P = cos_sin.shape[0]
+    with _Timed(tag, "rmsnorm_head72_rope"):
+        check(lib.mc_rmsnorm_head72_rope(x.data_ptr(), x.stride(0), x.shape[0], heads, weight.data_ptr(), eps,
+                                         cos_sin.data_ptr() if cos_sin is not None else None, int(pos_div), int(P), _stream()))
+    _count()
+    return x
+
+
+def attention_varlen_d72(q, k, v, heads, segs, max_q_len, scale=None, out=None, tag=None):
+    """softmax(q k^T * scale) v per head (head_dim 72) over independent segments in one launch (`mc_attn_varlen_d72`). q [Lq, H*72],
+    k / v [Lk, H*72] row-major bf16 views (row stride allowed); segs: int32 device tensor [n, 4] of (q_start, q_len, k_start, k_len)."""
+    _dev(q), _dev(k), _dev(v), _dev(segs, "segs")
+    assert q.dtype == k.dtype == v.dtype == torch.bfloat16 and q.stride(1) == 1 and k.stride(1) == 1 and v.stride(1) == 1
+    assert q.shape[1] == k.shape[1] == v.shape[1] == heads * 72 and k.shape[0] == v.shape[0]
+    assert segs.dtype == torch.int32 and segs.is_contiguous() and segs.dim() == 2 and segs.shape[1] == 4
+    if scale is None:
+        scale = 1.0 / math.sqrt(72)
+    if out is None:
+        out = torch.empty(q.shape[0], heads * 72, dtype=torch.bfloat16, device=q.device)
+    assert out.stride(1) == 1 and out.shape == q.shape
+    with _Timed(tag, "attn_varlen_d72"):
+        check(lib.mc_attn_varlen_d72(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), out.data_ptr(),
+                                     out.stride(0), heads, segs.data_ptr(), segs.shape[0], int(max_q_len), float(scale), _stream()))
+    _count()
+    return out
+
+
+def attention_temporal_d72(q, k, v, heads, B, T, S, scale=None, out=None, tag=None):
+    """Temporal attention (`mc_attn_temporal_d72`): rows in B (T S) C order, sequence (b, s) = rows b*T*S + t*S + s; head_dim 72."""
+    _dev(q), _dev(k), _dev(v)
+    for t_ in (q, k, v):
+        assert t_.dtype == torch.bfloat16 and t_.stride(1) == 1 and t_.shape == (B * T * S, heads * 72)
+    if scale is None:
+        scale = 1.0 / math.sqrt(72)
+    if out is None:
+        out = torch.empty(B * T * S, heads * 72, dtype=torch.bfloat16, device=q.device)
+    assert out.stride(1) == 1 and out.shape == q.shape
+    with _Timed(tag, "attn_temporal_d72"):
+        check(lib.mc_attn_temporal_d72(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), out.data_ptr(),
+                                       out.stride(0), B, T, S, heads, float(scale), _stream()))
+    _count()
+    return out
+
+
+def ln_t2i_modulate(x, em, scale_idx, shift_idx, eps=1e-6, out=None, tag=None):
+    """`t2i_modulate(LayerNorm(x), shift, scale)` with the bf16 rounding of every tensor op (`mc_ln_modulate` mode 2): x bf16
+    [rows, cols]; em fp32 [k, cols] holding bf16 values (scale row `scale_idx`, shift row `shift_idx`)."""
+    _dev(x)
+    rows, cols = x.shape
+    assert x.dtype == torch.bfloat16 and x.is_contiguous() and em.dtype == torch.float32 and em.is_contiguous() and em.shape[-1] == cols
+    if out is None:
+        out = torch.empty(rows, cols, dtype=torch.bfloat16, device=x.device)
+    assert out.dtype == torch.bfloat16 and out.is_contiguous() and out.shape == x.shape
+    with _Timed(tag, "ln_t2i_modulate"):
+        check(lib.mc_ln_modulate(x.data_ptr(), MC_BF16, rows, cols, eps, 2, em.data_ptr(), None, scale_idx, shift_idx, 0, out.data_ptr(),
+                                 MC_BF16, _stream()))
+    _count()
+    return out
+
+
 def colmean(x):
     """bf16 mean over the rows of a bf16 [rows, cols] view -> [1, cols] (torch semantics: bf16 sum, then bf16 division)."""
     _dev(x)

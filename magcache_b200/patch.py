@@ -562,6 +562,95 @@ def init_magcache_hunyuan(transformer, infer_steps=50, thresh=0.24, K=6, retenti
 
 
 # ------------------------------------------------------------------------------------------------------------------
+# Open-Sora 1.2 (STDiT3), the paper-evaluation forward behind the published Open-Sora numbers
+# ------------------------------------------------------------------------------------------------------------------
+def _opensora_unsupported(self, x_mask, kw):
+    if x_mask is not None:
+        raise NotImplementedError("magcache_b200: Open-Sora x_mask (image / video conditioning with t0) is not supported")
+    pm = getattr(self, "parallel_manager", None)
+    if pm is not None and (getattr(pm, "sp_size", 1) > 1 or getattr(pm, "cp_size", 1) > 1):
+        raise NotImplementedError("magcache_b200: Open-Sora sequence / CFG parallelism (sp_size or cp_size > 1) is not supported")
+    try:
+        from videosys.core.pab_mgr import enable_pab
+        pab = enable_pab()
+    except Exception:  # videosys absent or PAB never configured
+        pab = False
+    if pab:
+        raise NotImplementedError("magcache_b200: Open-Sora with PAB enabled is not supported")
+    if getattr(getattr(self, "config", None), "skip_y_embedder", False):
+        raise NotImplementedError("magcache_b200: Open-Sora with skip_y_embedder is not supported")
+
+
+def magcache_opensora_forward(self, x, timestep, all_timesteps, y, mask=None, x_mask=None, fps=None, height=None, width=None, **kw):
+    r"""eval/magcache/experiments/opensora.py:229-373 on the H100 kernels (magcache_b200/opensora.py), with the same signature and
+    class attributes (`t, skip_time, K, magcache_thresh, ratio, accumulated_sim / _err / _steps, skip_steps, residual_cache`).
+    The decision is the `"opensora"` controller family (`ratio[t-1]`, signed error, explicit `skip_time`), the counter wraps at 30
+    (:349-354) and the skip line of :312 is printed. `residual_cache` is the engine's one residual buffer viewed as (B, N, C, 1): the
+    reference's depth-3 FIFO is only ever read at [..., -1]; a tensor the caller puts there is honoured through its [..., -1].
+    Cross-attention follows `flash_attn_varlen_func`: each sample attends to its own `y_lens[b]` caption tokens (the default
+    `torch_impl` agrees whenever the lengths are equal, as for one prompt's CFG pair)."""
+    import ctypes
+
+    from . import _lib
+    from .config import FAMILIES
+    from .controller import make_ctrl_config
+    _opensora_unsupported(self, x_mask, kw)
+    if not x.is_cuda:
+        raise RuntimeError("magcache_b200: x must be a CUDA tensor (no CPU path)")
+    eng = self.__dict__.get("_mc_opensora_engine")
+    if eng is None:
+        from .opensora import OpenSoraEngine, OpenSoraWeights
+        eng = OpenSoraEngine(OpenSoraWeights.from_module(self, x.device))
+        object.__setattr__(self, "_mc_opensora_engine", eng)
+    eng.stage_inputs(x, timestep, y, mask, fps, height, width)
+    ratio = np.asarray(self.ratio, dtype=np.float64)
+    key = (hash(np.ascontiguousarray(ratio).tobytes()), len(ratio), float(self.magcache_thresh), int(self.K), int(self.skip_time))
+    cc = self.__dict__.get("_mc_opensora_cfg")
+    if cc is None or cc[0] != key:
+        kwf = dict(FAMILIES["opensora"], split_step=int(self.skip_time))
+        cc = (key, make_ctrl_config(30, self.magcache_thresh, self.K, 0.2, ratio, **kwf))
+        object.__setattr__(self, "_mc_opensora_cfg", cc)
+    skip_forward = False
+    if self.t >= self.skip_time:                       # :297-308
+        st = _lib.CtrlState()
+        st.cnt = int(self.t)
+        st.accumulated_ratio[0], st.accumulated_err[0], st.accumulated_steps[0] = float(self.accumulated_sim), float(self.accumulated_err), int(self.accumulated_steps)
+        st.accumulated_ratio[1] = 1.0
+        skip = ctypes.c_int32()
+        _lib.check(_lib.lib.mc_ctrl_decide(ctypes.byref(cc[1]), ctypes.byref(st), ctypes.byref(skip)))
+        self.accumulated_sim, self.accumulated_err, self.accumulated_steps = st.accumulated_ratio[0], st.accumulated_err[0], st.accumulated_steps[0]
+        skip_forward = bool(skip.value)
+    cur = self.residual_cache
+    if torch.is_tensor(cur) and cur.data_ptr() != eng.res.data_ptr():
+        eng.res.copy_(cur[..., -1].reshape(eng.res.shape))
+        eng.res_valid = True
+    if skip_forward:
+        self.skip_steps += 1
+        print(f"skip time {self.t}, cur_scale: {self.ratio[self.t-1]}, acc_sim: {self.accumulated_sim}, total_steps: {self.skip_steps}")  # :312
+    out = eng.forward("hit" if skip_forward else "miss")
+    self.residual_cache = eng.res.view(eng.B, eng.N, -1, 1)  # :344-347
+    self.t += 1                                        # :348-354
+    if self.t >= 30:
+        self.t = 0
+        self.accumulated_sim = 1.0
+        self.accumulated_steps = 0
+        self.accumulated_err = 0
+        self.skip_steps = 0
+    return out
+
+
+def init_magcache_opensora(transformer, thresh=0.12, K=3, skip_time=6, ratio=None):
+    """The installation block of `eval_ours` (opensora.py:418-436): the paper's presets are 0.12 / K3 and 0.24 / K5, skip_time 6."""
+    cls = transformer.__class__
+    cls.forward = magcache_opensora_forward
+    cls.magcache_thresh, cls.K, cls.skip_time = thresh, K, skip_time
+    cls.t, cls.residual_cache, cls.accumulated_err, cls.accumulated_sim, cls.accumulated_steps, cls.skip_steps = 0, None, 0, 1, 0, 0
+    cls.cache_time = 4
+    cls.ratio = np.asarray(tables()["opensora_eval"] if ratio is None else ratio, dtype=np.float64)
+    return transformer
+
+
+# ------------------------------------------------------------------------------------------------------------------
 # The paper-evaluation variant of the Wan forward (the code behind the published Wan2.1 numbers)
 # ------------------------------------------------------------------------------------------------------------------
 def magcache_eval_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
