@@ -8,6 +8,7 @@ from typing import Optional, Sequence
 import numpy as np
 
 from . import _lib
+from .controller import interp_cfg, make_ctrl_config, nearest_interp, nearest_interp_linspace, schedule_from
 
 _TABLES = None
 
@@ -59,38 +60,6 @@ def table_from_calibration(ratios, branches=2):
     if arr.ndim != 1 or len(arr) == 0 or not np.all(np.isfinite(arr)):
         raise ValueError("calibration ratios must be a non-empty 1-D list of finite numbers")
     return np.concatenate([np.ones(branches), arr])
-
-
-def nearest_interp(src, target_length):
-    """C-ABI `mc_nearest_interp` (MagCache4Wan2.1/magcache_generate.py:27-34)."""
-    import ctypes
-    src = np.ascontiguousarray(src, dtype=np.float64)
-    out = np.empty(target_length, dtype=np.float64)
-    dp = ctypes.POINTER(ctypes.c_double)
-    _lib.check(_lib.lib.mc_nearest_interp(src.ctypes.data_as(dp), len(src), out.ctypes.data_as(dp), target_length))
-    return out
-
-
-def interp_cfg(table, sample_steps):
-    """Per-CFG-branch interpolation (magcache_generate.py:915-919) through `mc_nearest_interp_cfg`."""
-    import ctypes
-    table = np.ascontiguousarray(table, dtype=np.float64)
-    if len(table) == 2 * sample_steps:
-        return table
-    out = np.empty(2 * sample_steps, dtype=np.float64)
-    dp = ctypes.POINTER(ctypes.c_double)
-    _lib.check(_lib.lib.mc_nearest_interp_cfg(table.ctypes.data_as(dp), len(table), out.ctypes.data_as(dp), sample_steps))
-    return out
-
-
-def nearest_interp_linspace(src, target_length):
-    """C-ABI `mc_nearest_interp_linspace`: Qwen-Image's form (MagCache4QwenImage/magcache_generate.py:14-21)."""
-    import ctypes
-    src = np.ascontiguousarray(src, dtype=np.float64)
-    out = np.empty(target_length, dtype=np.float64)
-    dp = ctypes.POINTER(ctypes.c_double)
-    _lib.check(_lib.lib.mc_nearest_interp_linspace(src.ctypes.data_as(dp), len(src), out.ctypes.data_as(dp), target_length))
-    return out
 
 
 # One row per adapter of the reference (SURVEY Appendix A): the controller parameters that differ between them.
@@ -178,21 +147,9 @@ class MagCacheConfig:
 
     def schedule(self, calls=None):
         """Skip mask (uint8 per forward call) of one video, from a fresh controller state."""
-        import ctypes
-
-        from .controller import make_ctrl_config
         R = 0.2 if self.family == "wan2.1-eval" else self.retention_ratio  # hard-coded upstream: `skip_time = int(self.num_steps*0.2)`, :772
         cfg = make_ctrl_config(self.num_steps, self.thresh, self.K, R, self.resolved_ratios(), **self.ctrl_kwargs())
-        calls = self.num_steps if calls is None else calls
-        st = _lib.CtrlState()
-        st.accumulated_ratio[0] = st.accumulated_ratio[1] = 1.0
-        st.accumulated_steps[0] = INITIAL_ACCUMULATED_STEPS.get(self.family, 0)
-        skip, out = ctypes.c_int32(), np.zeros(calls, dtype=np.uint8)
-        for i in range(calls):
-            _lib.check(_lib.lib.mc_ctrl_decide(ctypes.byref(cfg), ctypes.byref(st), ctypes.byref(skip)))
-            out[i] = skip.value
-            _lib.check(_lib.lib.mc_ctrl_advance(ctypes.byref(cfg), ctypes.byref(st)))
-        return out
+        return schedule_from(cfg, self.num_steps if calls is None else calls, INITIAL_ACCUMULATED_STEPS.get(self.family, 0))
 
 
 PRESETS = {

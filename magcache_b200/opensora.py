@@ -115,7 +115,9 @@ class OpenSoraEngine:
     """One STDiT3 on the sm_90a kernels. Buffers are allocated once per (B, T, H, W) shape; the caption buffer grows with the
     number of valid caption tokens."""
 
-    def __init__(self, weights: OpenSoraWeights):
+    def __init__(self, weights: OpenSoraWeights, shard_world=1, shard_rank=0, shard_group=None):
+        if shard_world > 1:  # no token-sharded path: every rank would compute the whole video
+            raise NotImplementedError("magcache_b200: Open-Sora token sharding (enable_token_shard with world > 1) is not supported")
         self.w, self.device = weights, weights.device
         self._shape = None
         self.res_valid = False

@@ -19,34 +19,32 @@ import numpy as np
 import torch
 
 from . import ops
-from .config import interp_cfg, table_for_ckpt_dir, tables
-from .controller import AttrController
+from .config import FAMILIES, interp_cfg, nearest_interp, save_json, table_for_ckpt_dir, table_from_calibration, tables
+from .controller import AttrController, TeaController
+from .mmdit import FluxEngine, FluxWeights, HunyuanEngine, HunyuanWeights
+from .opensora import OpenSoraEngine, OpenSoraWeights
 from .wan import WanEngine, WanWeights
 
-_WAN_CTRL = dict(branches=2, cmp=0, retention_mode=0, veto_index=-1, veto_base=0)  # `<`, int(n*R): magcache_generate.py:279-286
+# every engine a patched forward caches on its module (one per model family)
+ENGINE_ATTRS = ("_mc_engine", "_mc_flux_engine", "_mc_hunyuan_engine", "_mc_opensora_engine")
 
 
-def _engine(self):
-    eng = self.__dict__.get("_mc_engine")
+def _cached_engine(self, attr, build):
+    """The engine cached on the module under `attr` (one of ENGINE_ATTRS); on the first call `build(**shard_kw)` makes it, with the
+    keywords `enable_token_shard` left on the module."""
+    eng = self.__dict__.get(attr)
     if eng is None:
-        if hasattr(self, "patch_embedding"):
-            dev = self.patch_embedding.weight.device
-            if dev.type != "cuda":
-                raise RuntimeError("magcache_b200: the model must be on a CUDA device (no CPU path)")
-            weights = WanWeights.from_module(self, dev)
-        else:
-            raise TypeError("magcache_b200.magcache_forward expects a Wan2.1 WanModel (or an object carrying `_mc_engine`)")
-        eng = WanEngine(weights, **self.__dict__.get("_mc_shard_kw", {}))
-        object.__setattr__(self, "_mc_engine", eng)
+        eng = build(**self.__dict__.get("_mc_shard_kw", {}))
+        object.__setattr__(self, attr, eng)
     return eng
 
 
 def invalidate_engine(model):
     """Drop the engine cached on `model` (and with it the repacked bf16 copy of the weights, the workspaces and any captured CUDA
-    graphs). The engine snapshots the module's parameters at the first forward: call this after anything that changes them — a LoRA
-    merge, `load_state_dict`, `.to(...)` — and the next forward repacks. The module's own parameters stay resident next to the
-    packed copy (about +2.8 GB for the 1.3B model, +28 GB for 14B); free or offload them yourself if that matters."""
-    for name in ("_mc_engine", "_mc_flux_engine", "_mc_hunyuan_engine", "_mc_ctrl"):
+    graphs) and its controllers. The engine snapshots the module's parameters at the first forward: call this after anything that
+    changes them — a LoRA merge, `load_state_dict`, `.to(...)` — and the next forward repacks. The module's own parameters stay
+    resident next to the packed copy (about +2.8 GB for the 1.3B model, +28 GB for 14B); free or offload them yourself if that matters."""
+    for name in ENGINE_ATTRS + ("_mc_ctrls",):
         model.__dict__.pop(name, None)
     return model
 
@@ -55,19 +53,79 @@ def enable_token_shard(model, rank, world, group=None):
     """Shard the token axis of `model`'s forwards over `world` ranks of one node (call before the first forward; needs an
     initialised torch.distributed NCCL group). Every rank must then make the same calls with the same inputs; outputs are
     replicated, the residual cache stays sharded. Wan engines shard all tokens; the FLUX / HunyuanVideo engines shard the image tokens and
-    replicate the text tokens."""
-    if any(k in model.__dict__ for k in ("_mc_engine", "_mc_flux_engine", "_mc_hunyuan_engine")):
+    replicate the text tokens. The Open-Sora engine has no sharded path: its forward raises NotImplementedError for world > 1."""
+    if any(k in model.__dict__ for k in ENGINE_ATTRS):
         raise RuntimeError("enable_token_shard must be called before the first forward")
     object.__setattr__(model, "_mc_shard_kw", dict(shard_world=world, shard_rank=rank, shard_group=group))
     return model
 
 
-def _controller(self):
-    c = self.__dict__.get("_mc_ctrl")
+# the paper-evaluation scripts keep the controller inputs under their own attribute names and hard-code some of them
+_ATTR_NAMES = {
+    # eval/magcache/experiments/Wan2.1_EVAL/wan_magcache.py:770-786 (`skip_time = int(self.num_steps*0.2)`, :772)
+    "wan2.1-eval": (dict(cnt="t", K="magcache_K", mag_ratios="ratio", accumulated_ratio="accumulated_sim"), dict(retention_ratio=0.2)),
+    # eval/magcache/experiments/opensora.py:297-308 (30 steps per video, :349-354)
+    "opensora": (dict(cnt="t", mag_ratios="ratio", accumulated_ratio="accumulated_sim", split_step="skip_time"),
+                 dict(num_steps=30, retention_ratio=0.2)),
+}
+
+
+def _ctrl(self, family):
+    """The module's controller for `family` (a key of `config.FAMILIES`)."""
+    ctrls = self.__dict__.setdefault("_mc_ctrls", {})
+    c = ctrls.get(family)
     if c is None:
-        c = AttrController(_WAN_CTRL)
-        object.__setattr__(self, "_mc_ctrl", c)
+        c = ctrls[family] = AttrController(FAMILIES[family], *_ATTR_NAMES.get(family, ()))
     return c
+
+
+def _take_residual(eng, cur, slot=None):
+    """The reference keeps the cached residual in an attribute (`cur`, its current value); the engine keeps it in a fixed buffer that
+    the attribute aliases (`eng.res`, or `eng.res[slot]` for the per-CFG-branch engines). If a caller replaced the attribute (or
+    cleared it), follow the attribute."""
+    res = eng.res if slot is None else eng.res[slot]
+    if cur is None:
+        valid = False
+    elif torch.is_tensor(cur) and cur.data_ptr() != res.data_ptr():
+        res.copy_(cur.reshape(res.shape))
+        valid = True
+    else:
+        return
+    if slot is None:
+        eng.res_valid = valid
+    else:
+        eng.res_valid[slot] = valid
+
+
+def _record_stats(self, stats):
+    """One calibration call's statistics: appended rounded to 5 places and printed like the reference."""
+    norm_ratio, norm_std, cos_dis = stats
+    self.norm_ratio.append(round(norm_ratio, 5))
+    self.norm_std.append(round(norm_std, 5))
+    self.cos_dis.append(round(cos_dis, 5))
+    print(f"time: {self.cnt}, norm_ratio: {norm_ratio}, norm_std: {norm_std}, cos_dis: {cos_dis}")
+
+
+def _print_stats(self):
+    print("norm ratio")
+    print(self.norm_ratio)
+    print("norm std")
+    print(self.norm_std)
+    print("cos_dis")
+    print(self.cos_dis)
+
+
+def _wan_weights(self):
+    if not hasattr(self, "patch_embedding"):
+        raise TypeError("magcache_b200.magcache_forward expects a Wan2.1 WanModel (or an object carrying `_mc_engine`)")
+    dev = self.patch_embedding.weight.device
+    if dev.type != "cuda":
+        raise RuntimeError("magcache_b200: the model must be on a CUDA device (no CPU path)")
+    return WanWeights.from_module(self, dev)
+
+
+def _engine(self):
+    return _cached_engine(self, "_mc_engine", lambda **kw: WanEngine(_wan_weights(self), **kw))
 
 
 def _stage(self, x, t, context, seq_len, clip_fea, y, pad_ok=True, vace_context=None, vace_scale=1.0, require_clip=True):
@@ -95,17 +153,6 @@ def _stage(self, x, t, context, seq_len, clip_fea, y, pad_ok=True, vace_context=
     return eng
 
 
-def _sync_slot_in(self, eng, slot):
-    """The reference keeps the cached residual in `self.residual_cache[slot]`; the engine keeps it in a fixed buffer that the
-    attribute aliases. If a caller replaced the attribute (or cleared it), follow the attribute."""
-    cur = self.residual_cache[slot]
-    if cur is None:
-        eng.res_valid[slot] = False
-    elif torch.is_tensor(cur) and cur.data_ptr() != eng.res[slot].data_ptr():
-        eng.res[slot].copy_(cur.reshape(eng.res[slot].shape))
-        eng.res_valid[slot] = True
-
-
 def magcache_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
     r"""MagCache4Wan2.1/magcache_generate.py:198-312 on the H100 kernels.
 
@@ -113,10 +160,10 @@ def magcache_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
     -> List[Tensor[C_out, F, H, W]] (float32).
     """
     eng = _stage(self, x, t, context, seq_len, clip_fea, y)
-    ctrl = _controller(self)
+    ctrl = _ctrl(self, "wan2.1")
     slot = self.cnt % 2
     skip_forward = ctrl.decide(self)  # :279-292 (float64 state under the reference's attribute names)
-    _sync_slot_in(self, eng, slot)
+    _take_residual(eng, self.residual_cache[slot], slot)
     # hit : `x = x + residual_x` (:295) feeds only the head, so the sum is formed inside the head kernel (same fp32 arithmetic)
     # miss: block stack (:297-298), `residual_x = x - ori_x` (:299) written into the slot's buffer
     out = eng.forward("hit" if skip_forward else "miss", slot)
@@ -131,10 +178,10 @@ def magcache_vace_forward(self, x, t, vace_context, context, seq_len, vace_conte
     every second main block adds its hint; on a hit nothing of the control branch is computed, as in the reference. `clip_fea` and
     `y` are accepted and ignored (the reference has those lines commented out, :471-476, :505-507)."""
     eng = _stage(self, x, t, context, seq_len, None, None, vace_context=vace_context, vace_scale=vace_context_scale)
-    ctrl = _controller(self)
+    ctrl = _ctrl(self, "wan2.1")
     slot = self.cnt % 2
     skip_forward = ctrl.decide(self)  # :517-531
-    _sync_slot_in(self, eng, slot)
+    _take_residual(eng, self.residual_cache[slot], slot)
     if skip_forward:
         print("skip: ", self.cnt)  # :527
     out = eng.forward("hit" if skip_forward else "miss", slot)
@@ -164,15 +211,10 @@ def magcache_wan22_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
             raise NotImplementedError("magcache_b200: one sample per call")
         assert t.size(1) == seq_len  # what `.unflatten(0, (bt, seq_len))` (:270) requires
     eng = _stage(self, x, t, context, seq_len, None, y, require_clip=False)
-    ctrls = self.__dict__.setdefault("_mc_ctrls", {})
-    fam = "wan2.2-i2v" if getattr(self, "mode", "t2v") == "i2v" else "wan2.2-t2v"
-    if fam not in ctrls:
-        from .config import FAMILIES
-        ctrls[fam] = AttrController(FAMILIES[fam])
-    ctrl = ctrls[fam]
+    ctrl = _ctrl(self, "wan2.2-i2v" if getattr(self, "mode", "t2v") == "i2v" else "wan2.2-t2v")
     slot = int(self.cnt) % 2
     skip_forward = ctrl.decide(self)  # :290-317
-    _sync_slot_in(self, eng, slot)    # the other expert's residual arrives through the shared class-level list
+    _take_residual(eng, self.residual_cache[slot], slot)  # the other expert's residual arrives through the shared class-level list
     out = eng.forward("hit" if skip_forward else "miss", slot)
     self.residual_cache[slot] = eng.res[slot].view(1, *eng.res[slot].shape)  # :324
     ctrl.advance(self)  # :328-334
@@ -183,7 +225,6 @@ def init_magcache_wan22(model, mag_ratios, sample_steps, thresh=0.06, K=2, reten
     """`init_magcache(model, mag_ratios, args, split_steps, mode)` of MagCache4Wan2.2/magcache_generate.py:340-362: patches the CLASS the
     two experts share. `mag_ratios`: the list without its `[1.0]*2` prefix like the script passes it, or a key of `tables()` (which
     already carries the prefix)."""
-    import numpy as np
     cls = model.__class__
     cls.forward = magcache_wan22_forward
     cls.cnt = torch.tensor(0)
@@ -206,52 +247,22 @@ def magcache_calibration(self, x, t, context, seq_len, clip_fea=None, y=None):
 
 
 def _calibrate(self, eng):
-    x0, e, e0, ctx = eng.prologue()
-    xs = eng.run_blocks(x0, e0, ctx, eng.grid)
     slot = self.cnt % 2
-    if self.cnt >= 2:
-        prev = self.residual_cache[slot].view(x0.shape)
-        reduce = None
-        if eng.shard is not None:  # the statistics are sums over tokens: add the partial sums of every token shard
-            from .shard import allreduce_stats
-            reduce = lambda st: allreduce_stats(st, eng.shard.group)  # noqa: E731
-        if eng.pad_row:
-            # seq_len > token count: rows [n_tok, seq_len) of the reference's tensors are identical copies of the one pad row computed
-            # here; its three per-row terms enter the means (seq_len - n_tok) times (:167-169 average over dim 1 of [1, seq_len, D])
-            n_tok, wgt = eng.n_keys, float(eng.pad_weight)
-            keep = {}
-            ops.residual_sub_stats(xs[n_tok:], x0[n_tok:], prev[n_tok:].contiguous(), reduce=lambda st: keep.setdefault("pad", st.clone()))
-            residual_tok, (norm_ratio, norm_std, cos_dis) = ops.residual_sub_stats(
-                xs[:n_tok], x0[:n_tok], prev[:n_tok].contiguous(), reduce=lambda st: st + keep["pad"] * st.new_tensor([wgt, wgt, wgt, wgt]))
-            residual_x = torch.cat([residual_tok, xs[n_tok:] - x0[n_tok:].float()])
-        else:
-            residual_x, (norm_ratio, norm_std, cos_dis) = ops.residual_sub_stats(xs, x0, prev, reduce=reduce)
-        self.norm_ratio.append(round(norm_ratio, 5))
-        self.norm_std.append(round(norm_std, 5))
-        self.cos_dis.append(round(cos_dis, 5))
-        print(f"time: {self.cnt}, norm_ratio: {norm_ratio}, norm_std: {norm_std}, cos_dis: {cos_dis}")
-    else:
-        residual_x = ops.residual_sub(xs, x0)
-    self.residual_cache[slot] = residual_x.view(1, *x0.shape)
-    eng._slot = slot
-    out = eng.head(xs, e, eng.grid)
+    out, stats = eng.calibrate(slot, self.residual_cache[slot] if self.cnt >= 2 else None)
+    if stats is not None:
+        _record_stats(self, stats)
+    self.residual_cache[slot] = eng.cal_residual
     self.cnt += 1
     if self.cnt >= self.num_steps:
         self.cnt = 0
         self.accumulated_ratio = [1.0, 1.0]
         self.accumulated_err = [0.0, 0.0]
         self.accumulated_steps = [0, 0]
-        print("norm ratio")
-        print(self.norm_ratio)
-        print("norm std")
-        print(self.norm_std)
-        print("cos_dis")
-        print(self.cos_dis)
+        _print_stats(self)
         # :191-193 `save_json("wan2_1_mag_ratio", self.norm_ratio)` ...: same file names, in `calibration_dir` (default: the
         # working directory, like the reference). `config.table_from_calibration` turns the first file into a `mag_ratios` table.
         out_dir = getattr(self, "calibration_dir", ".")
         if out_dir is not None:
-            from .config import save_json
             save_json(os.path.join(out_dir, "wan2_1_mag_ratio"), self.norm_ratio)
             save_json(os.path.join(out_dir, "wan2_1_mag_std"), self.norm_std)
             save_json(os.path.join(out_dir, "wan2_1_cos_dis"), self.cos_dis)
@@ -274,7 +285,6 @@ def init_magcache(model, sample_steps, thresh=0.12, K=2, retention_ratio=0.2, ma
     cls.retention_ratio = retention_ratio
     cls.residual_cache = [None, None]
     if isinstance(mag_ratios, (str, os.PathLike)):  # a calibration dump (`wan2_1_mag_ratio.json`) instead of a pasted literal
-        from .config import table_from_calibration
         mag_ratios = table_from_calibration(mag_ratios)
     if mag_ratios is None:
         mag_ratios = tables()[table] if table is not None else table_for_ckpt_dir(ckpt_dir)
@@ -318,11 +328,7 @@ def magcache_branch(self, hidden, run_blocks, family, cache_attr):
     the cached residual (K1 kernel) or calls `run_blocks(hidden)` (the model's own transformer stack) and stores `out - hidden`
     (K2 kernel) under `cache_attr` — a tensor for scalar-state families, a 2-list indexed by `cnt % 2` for per-branch ones.
     Advances the counter. Wan2.2's expert boundary is read from `self.split_step` like upstream (:344)."""
-    from .config import FAMILIES
-    ctrls = self.__dict__.setdefault("_mc_ctrls", {})
-    if family not in ctrls:
-        ctrls[family] = AttrController(FAMILIES[family])
-    ctrl = ctrls[family]
+    ctrl = _ctrl(self, family)
     per_branch = FAMILIES[family]["branches"] == 2
     slot = int(self.cnt) % 2 if per_branch else None
     if ctrl.decide(self):
@@ -351,34 +357,32 @@ class _Sample:
         self.sample = sample
 
 
+def _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance, joint_attention_kwargs,
+                controlnet_block_samples, controlnet_single_block_samples):
+    if joint_attention_kwargs or controlnet_block_samples is not None or controlnet_single_block_samples is not None:
+        raise NotImplementedError("magcache_b200: joint_attention_kwargs / ControlNet residuals are not built for the FLUX engine")
+    if not hidden_states.is_cuda:
+        raise RuntimeError("magcache_b200: hidden_states must be CUDA tensors (no CPU path)")
+    eng = _cached_engine(self, "_mc_flux_engine", lambda **kw: FluxEngine(FluxWeights.from_module(self, hidden_states.device), **kw))
+    if txt_ids.ndim == 3:  # :305-316 (deprecated 3-D ids)
+        txt_ids = txt_ids[0]
+    if img_ids.ndim == 3:
+        img_ids = img_ids[0]
+    eng.stage_inputs(hidden_states, encoder_hidden_states, pooled_projections, timestep, guidance, img_ids, txt_ids)
+    return eng
+
+
 def magcache_flux_forward(self, hidden_states, encoder_hidden_states=None, pooled_projections=None, timestep=None, img_ids=None,
                           txt_ids=None, guidance=None, joint_attention_kwargs=None, controlnet_block_samples=None,
                           controlnet_single_block_samples=None, return_dict=True, controlnet_blocks_repeat=False):
     r"""MagCache4FLUX/magcache_flux.py:234-440 on the H100 kernels: same signature, same state attributes (`cnt, num_steps,
     magcache_thresh, K, retention_ratio, accumulated_ratio / _err / _steps, previous_residual, mag_ratios`), `(output,)` or an object
     with `.sample`. LoRA scaling, ip-adapter and ControlNet residuals (:275-288, :321-324, :371-381, :410-420) are not built and raise."""
-    if joint_attention_kwargs or controlnet_block_samples is not None or controlnet_single_block_samples is not None:
-        raise NotImplementedError("magcache_b200: joint_attention_kwargs / ControlNet residuals are not built for the FLUX engine")
-    if not hidden_states.is_cuda:
-        raise RuntimeError("magcache_b200: hidden_states must be CUDA tensors (no CPU path)")
-    eng = _flux_engine(self, hidden_states)
-    if txt_ids.ndim == 3:  # :305-316 (deprecated 3-D ids)
-        txt_ids = txt_ids[0]
-    if img_ids.ndim == 3:
-        img_ids = img_ids[0]
-    eng.stage_inputs(hidden_states, encoder_hidden_states, pooled_projections, timestep, guidance, img_ids, txt_ids)
-    ctrls = self.__dict__.setdefault("_mc_ctrls", {})
-    if "flux" not in ctrls:
-        from .config import FAMILIES
-        ctrls["flux"] = AttrController(FAMILIES["flux"])
-    ctrl = ctrls["flux"]
+    eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
+                      joint_attention_kwargs, controlnet_block_samples, controlnet_single_block_samples)
+    ctrl = _ctrl(self, "flux")
     skip_forward = ctrl.decide(self)  # :326-338
-    cur = self.previous_residual
-    if cur is None:
-        eng.res_valid = False
-    elif torch.is_tensor(cur) and cur.data_ptr() != eng.res.data_ptr():
-        eng.res.copy_(cur.reshape(eng.res.shape))
-        eng.res_valid = True
+    _take_residual(eng, self.previous_residual)
     out = eng.forward("hit" if skip_forward else "miss")
     self.previous_residual = eng.res.view(1, *eng.res.shape)  # :427
     ctrl.advance(self)  # :431-436
@@ -388,45 +392,22 @@ def magcache_flux_forward(self, hidden_states, encoder_hidden_states=None, poole
     return _Sample(output)
 
 
-def _flux_engine(self, hidden_states):
-    eng = self.__dict__.get("_mc_flux_engine")
-    if eng is None:
-        from .mmdit import FluxEngine, FluxWeights
-        eng = FluxEngine(FluxWeights.from_module(self, hidden_states.device), **self.__dict__.get("_mc_shard_kw", {}))
-        object.__setattr__(self, "_mc_flux_engine", eng)
-    return eng
-
-
 def magcache_flux_calibration(self, hidden_states, encoder_hidden_states=None, pooled_projections=None, timestep=None, img_ids=None,
                               txt_ids=None, guidance=None, joint_attention_kwargs=None, controlnet_block_samples=None,
                               controlnet_single_block_samples=None, return_dict=True, controlnet_blocks_repeat=False):
     r"""MagCache4FLUX/magcache_flux.py:21-231: every call runs the block stack and, from the second call on, records the token-mean
     magnitude ratio, its std and the cosine distance to the previous residual (`norm_ratio / norm_std / cos_dis`, rounded to 5 places);
     the lists are printed on the last call of a generation and cleared at the wrap (:207-221)."""
-    if joint_attention_kwargs or controlnet_block_samples is not None or controlnet_single_block_samples is not None:
-        raise NotImplementedError("magcache_b200: joint_attention_kwargs / ControlNet residuals are not built for the FLUX engine")
-    if not hidden_states.is_cuda:
-        raise RuntimeError("magcache_b200: hidden_states must be CUDA tensors (no CPU path)")
-    eng = _flux_engine(self, hidden_states)
-    eng.stage_inputs(hidden_states, encoder_hidden_states, pooled_projections, timestep, guidance,
-                     img_ids[0] if img_ids.ndim == 3 else img_ids, txt_ids[0] if txt_ids.ndim == 3 else txt_ids)
+    eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
+                      joint_attention_kwargs, controlnet_block_samples, controlnet_single_block_samples)
     if self.cnt == 0:
         eng.res_valid = False  # `if self.cnt>=1` (:199): the first call of a generation has nothing to compare with
     out, stats = eng.calibrate()
-    if self.cnt >= 1 and stats is not None:
-        norm_ratio, norm_std, cos_dis = stats
-        self.norm_ratio.append(round(norm_ratio, 5))
-        self.norm_std.append(round(norm_std, 5))
-        self.cos_dis.append(round(cos_dis, 5))
-        print(f"time: {self.cnt}, norm_ratio: {norm_ratio}, norm_std: {norm_std}, cos_dis: {cos_dis}")
+    if stats is not None:
+        _record_stats(self, stats)
     self.previous_residual = eng.res.view(1, *eng.res.shape)
     if self.cnt >= self.num_steps - 1:
-        print("norm ratio")
-        print(self.norm_ratio)
-        print("norm std")
-        print(self.norm_std)
-        print("cos_dis")
-        print(self.cos_dis)
+        _print_stats(self)
     self.cnt += 1
     if self.cnt >= self.num_steps:
         self.cnt = 0
@@ -448,8 +429,6 @@ def init_magcache_flux_calibration(transformer, num_inference_steps=28):
 def init_magcache_flux(transformer, num_inference_steps=28, thresh=0.24, K=5, retention_ratio=0.1, mag_ratios=None, table="flux_dev"):
     """The installation statements of magcache_flux.py:446-471 (Kontext: magcache_flux_kontext.py:445-470 with table "flux_kontext",
     thresh 0.05, K 4, retention 0.2): patches the CLASS."""
-    from .config import nearest_interp
-    import numpy as np
     cls = transformer.__class__
     cls.forward = magcache_flux_forward
     cls.cnt, cls.num_steps = 0, num_inference_steps
@@ -463,32 +442,24 @@ def init_magcache_flux(transformer, num_inference_steps=28, thresh=0.24, K=5, re
     return transformer
 
 
+def _hunyuan_stage(self, x, t, text_states, text_mask, text_states_2, freqs_cos, freqs_sin, guidance):
+    if not x.is_cuda:
+        raise RuntimeError("magcache_b200: x must be a CUDA tensor (no CPU path)")
+    eng = _cached_engine(self, "_mc_hunyuan_engine", lambda **kw: HunyuanEngine(HunyuanWeights.from_module(self, x.device), **kw))
+    eng.stage_inputs(x, t, text_states, text_mask, text_states_2, freqs_cos, freqs_sin, guidance)
+    return eng
+
+
 def magcache_hunyuan_forward(self, x, t, text_states=None, text_mask=None, text_states_2=None, freqs_cos=None, freqs_sin=None,
                              guidance=None, return_dict=True):
     r"""MagCache4HunyuanVideo/magcache_sample_video.py:29-160 on the H100 kernels (MMDiT engine, magcache_b200/mmdit.py; opt-in until
     validated on a GPU): same signature and state attributes (`cnt, num_steps, magcache_thresh, K, retention_ratio, accumulated_ratio /
     _err / _steps, residual_cache, mag_ratios`), returns `{"x": img}` or the tensor. x [1, 16, T, H, W]; text_mask marks the valid
     (right-padded) text tokens."""
-    if not x.is_cuda:
-        raise RuntimeError("magcache_b200: x must be a CUDA tensor (no CPU path)")
-    eng = self.__dict__.get("_mc_hunyuan_engine")
-    if eng is None:
-        from .mmdit import HunyuanEngine, HunyuanWeights
-        eng = HunyuanEngine(HunyuanWeights.from_module(self, x.device), **self.__dict__.get("_mc_shard_kw", {}))
-        object.__setattr__(self, "_mc_hunyuan_engine", eng)
-    eng.stage_inputs(x, t, text_states, text_mask, text_states_2, freqs_cos, freqs_sin, guidance)
-    ctrls = self.__dict__.setdefault("_mc_ctrls", {})
-    if "hunyuan" not in ctrls:
-        from .config import FAMILIES
-        ctrls["hunyuan"] = AttrController(FAMILIES["hunyuan"])
-    ctrl = ctrls["hunyuan"]
+    eng = _hunyuan_stage(self, x, t, text_states, text_mask, text_states_2, freqs_cos, freqs_sin, guidance)
+    ctrl = _ctrl(self, "hunyuan")
     skip_forward = ctrl.decide(self)  # :88-102
-    cur = self.residual_cache
-    if cur is None:
-        eng.res_valid = False
-    elif torch.is_tensor(cur) and cur.data_ptr() != eng.res.data_ptr():
-        eng.res.copy_(cur.reshape(eng.res.shape))
-        eng.res_valid = True
+    _take_residual(eng, self.residual_cache)
     img = eng.forward("hit" if skip_forward else "miss")
     self.residual_cache = eng.res.view(1, *eng.res.shape)  # :141
     ctrl.advance(self)  # :149-154
@@ -501,31 +472,15 @@ def magcache_hunyuan_calibration(self, x, t, text_states=None, text_mask=None, t
                                  guidance=None, return_dict=True):
     r"""MagCache4HunyuanVideo/magcache_sample_video.py:163-290: the calibration twin (statistics from the second call on, lists printed
     from call 49 on — hard-coded upstream, :266 — and a counter that is never wrapped, :281)."""
-    if not x.is_cuda:
-        raise RuntimeError("magcache_b200: x must be a CUDA tensor (no CPU path)")
-    eng = self.__dict__.get("_mc_hunyuan_engine")
-    if eng is None:
-        from .mmdit import HunyuanEngine, HunyuanWeights
-        eng = HunyuanEngine(HunyuanWeights.from_module(self, x.device))
-        object.__setattr__(self, "_mc_hunyuan_engine", eng)
-    eng.stage_inputs(x, t, text_states, text_mask, text_states_2, freqs_cos, freqs_sin, guidance)
+    eng = _hunyuan_stage(self, x, t, text_states, text_mask, text_states_2, freqs_cos, freqs_sin, guidance)
     if self.cnt == 0:
         eng.res_valid = False
     img, stats = eng.calibrate()
-    if self.cnt >= 1 and stats is not None:
-        norm_ratio, norm_std, cos_dis = stats
-        self.norm_ratio.append(round(norm_ratio, 5))
-        self.norm_std.append(round(norm_std, 5))
-        self.cos_dis.append(round(cos_dis, 5))
-        print(f"time: {self.cnt}, norm_ratio: {norm_ratio}, norm_std: {norm_std}, cos_dis: {cos_dis}")
+    if stats is not None:
+        _record_stats(self, stats)
     self.residual_cache = eng.res.view(1, *eng.res.shape)
     if self.cnt >= 49:
-        print("norm ratio")
-        print(self.norm_ratio)
-        print("norm std")
-        print(self.norm_std)
-        print("cos_dis")
-        print(self.cos_dis)
+        _print_stats(self)
     self.cnt += 1
     return {"x": img} if return_dict else img
 
@@ -542,9 +497,6 @@ def init_magcache_hunyuan_calibration(transformer, infer_steps=50):
 
 def init_magcache_hunyuan(transformer, infer_steps=50, thresh=0.24, K=6, retention_ratio=0.2, video_height=720, mag_ratios=None):
     """The installation statements of magcache_sample_video.py:303-328 (table chosen by `args.video_size[0]` in {720, 544}, :315-318)."""
-    import numpy as np
-
-    from .config import nearest_interp
     cls = transformer.__class__
     cls.cnt, cls.num_steps, cls.magcache_thresh, cls.K = 0, infer_steps, thresh, K
     cls.residual_cache = None
@@ -589,41 +541,14 @@ def magcache_opensora_forward(self, x, timestep, all_timesteps, y, mask=None, x_
     reference's depth-3 FIFO is only ever read at [..., -1]; a tensor the caller puts there is honoured through its [..., -1].
     Cross-attention follows `flash_attn_varlen_func`: each sample attends to its own `y_lens[b]` caption tokens (the default
     `torch_impl` agrees whenever the lengths are equal, as for one prompt's CFG pair)."""
-    import ctypes
-
-    from . import _lib
-    from .config import FAMILIES
-    from .controller import make_ctrl_config
     _opensora_unsupported(self, x_mask, kw)
     if not x.is_cuda:
         raise RuntimeError("magcache_b200: x must be a CUDA tensor (no CPU path)")
-    eng = self.__dict__.get("_mc_opensora_engine")
-    if eng is None:
-        from .opensora import OpenSoraEngine, OpenSoraWeights
-        eng = OpenSoraEngine(OpenSoraWeights.from_module(self, x.device))
-        object.__setattr__(self, "_mc_opensora_engine", eng)
+    eng = _cached_engine(self, "_mc_opensora_engine", lambda **skw: OpenSoraEngine(OpenSoraWeights.from_module(self, x.device), **skw))
     eng.stage_inputs(x, timestep, y, mask, fps, height, width)
-    ratio = np.asarray(self.ratio, dtype=np.float64)
-    key = (hash(np.ascontiguousarray(ratio).tobytes()), len(ratio), float(self.magcache_thresh), int(self.K), int(self.skip_time))
-    cc = self.__dict__.get("_mc_opensora_cfg")
-    if cc is None or cc[0] != key:
-        kwf = dict(FAMILIES["opensora"], split_step=int(self.skip_time))
-        cc = (key, make_ctrl_config(30, self.magcache_thresh, self.K, 0.2, ratio, **kwf))
-        object.__setattr__(self, "_mc_opensora_cfg", cc)
-    skip_forward = False
-    if self.t >= self.skip_time:                       # :297-308
-        st = _lib.CtrlState()
-        st.cnt = int(self.t)
-        st.accumulated_ratio[0], st.accumulated_err[0], st.accumulated_steps[0] = float(self.accumulated_sim), float(self.accumulated_err), int(self.accumulated_steps)
-        st.accumulated_ratio[1] = 1.0
-        skip = ctypes.c_int32()
-        _lib.check(_lib.lib.mc_ctrl_decide(ctypes.byref(cc[1]), ctypes.byref(st), ctypes.byref(skip)))
-        self.accumulated_sim, self.accumulated_err, self.accumulated_steps = st.accumulated_ratio[0], st.accumulated_err[0], st.accumulated_steps[0]
-        skip_forward = bool(skip.value)
+    skip_forward = self.t >= self.skip_time and _ctrl(self, "opensora").decide(self)  # :297-308
     cur = self.residual_cache
-    if torch.is_tensor(cur) and cur.data_ptr() != eng.res.data_ptr():
-        eng.res.copy_(cur[..., -1].reshape(eng.res.shape))
-        eng.res_valid = True
+    _take_residual(eng, cur[..., -1] if torch.is_tensor(cur) else cur)
     if skip_forward:
         self.skip_steps += 1
         print(f"skip time {self.t}, cur_scale: {self.ratio[self.t-1]}, acc_sim: {self.accumulated_sim}, total_steps: {self.skip_steps}")  # :312
@@ -660,34 +585,14 @@ def magcache_eval_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
     retention fixed at `int(num_steps*0.2)`, residuals kept from call 10 on (`cache_time`) in a `[2, B, N, D, 1]` tensor — the
     depth-1 `push_tensor_roll` FIFO (:67-85, :796-799) is the engine's two residual slots viewed in place, no roll, no copy —
     and the conditional output of each step remembered in `pre_con` (:804-805)."""
-    import ctypes
-
-    from . import _lib
-    from .config import FAMILIES
-    from .controller import make_ctrl_config
     eng = _stage(self, x, t, context, seq_len, clip_fea, y)
     cache_time = 10                                  # :771
-    ratio = self.ratio
-    cc = self.__dict__.get("_mc_eval_cfg")
-    key = (hash(np.ascontiguousarray(np.asarray(ratio, dtype=np.float64)).tobytes()), len(ratio), self.num_steps, float(self.magcache_thresh),
-           int(self.magcache_K))
-    if cc is None or cc[0] != key:
-        cc = (key, make_ctrl_config(self.num_steps, self.magcache_thresh, self.magcache_K, 0.2, ratio, **FAMILIES["wan2.1-eval"]))
-        object.__setattr__(self, "_mc_eval_cfg", cc)
-    cfg = cc[1]
-    st = _lib.CtrlState()
-    st.cnt = int(self.t)
-    for i in range(2):
-        st.accumulated_ratio[i], st.accumulated_err[i], st.accumulated_steps[i] = float(self.accumulated_sim[i]), float(self.accumulated_err[i]), int(self.accumulated_steps[i])
-    skip = ctypes.c_int32()
-    _lib.check(_lib.lib.mc_ctrl_decide(ctypes.byref(cfg), ctypes.byref(st), ctypes.byref(skip)))  # :774-786
-    for i in range(2):  # the reference mutates the lists in place
-        self.accumulated_sim[i], self.accumulated_err[i], self.accumulated_steps[i] = st.accumulated_ratio[i], st.accumulated_err[i], st.accumulated_steps[i]
+    skip_forward = _ctrl(self, "wan2.1-eval").decide(self)  # :774-786
     slot = self.t % 2
-    if skip.value:
+    if skip_forward:
         self.skip_steps += 1
-        print(f"skip time {self.t}, cur_scale: {ratio[self.t - 10]}, acc_sim: {self.accumulated_sim[slot]}, total_steps: {self.skip_steps}")  # :790
-    out = eng.forward("hit" if skip.value else "miss", slot)
+        print(f"skip time {self.t}, cur_scale: {self.ratio[self.t - 10]}, acc_sim: {self.accumulated_sim[slot]}, total_steps: {self.skip_steps}")  # :790
+    out = eng.forward("hit" if skip_forward else "miss", slot)
     if self.t >= cache_time:                         # :796-799
         self.residual_cache = eng.res_buf.view(2, 1, *eng.res_buf.shape[1:], 1)
     if self.t % 2 == 0:
@@ -704,7 +609,6 @@ def magcache_eval_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
 
 def init_magcache_eval(model, sample_steps, thresh=0.12, K=2, ratio=None):
     """The installation block of wan_magcache.py:1129-1150 as a helper ("slow" = 0.12/K2, "fast" = 0.12/K4, wan_eval.sh:30-31,66-67)."""
-    import numpy as np
     cls = model.__class__
     cls.forward = magcache_eval_forward
     cls.magcache_thresh, cls.magcache_K = thresh, K
@@ -728,19 +632,7 @@ TEACACHE_COEFFICIENTS = {
 }
 
 
-def _tea_structs(self):
-    import ctypes
-
-    from . import _lib
-    coef = [float(c) for c in self.coefficients]
-    cfg = _lib.TeaConfig()
-    cfg.num_steps, cfg.ret_steps, cfg.cutoff_steps, cfg.n_coef, cfg.thresh = int(self.num_steps), int(self.ret_steps), int(self.cutoff_steps), len(coef), float(self.teacache_thresh)
-    for i, c in enumerate(coef):
-        cfg.coef[i] = c
-    st = _lib.TeaState()
-    st.cnt = int(self.cnt)
-    st.accumulated[0], st.accumulated[1] = float(self.accumulated_rel_l1_distance_even), float(self.accumulated_rel_l1_distance_odd)
-    return ctypes, _lib, cfg, st
+_TEA = TeaController()
 
 
 def teacache_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
@@ -754,32 +646,21 @@ def teacache_forward(self, x, t, context, seq_len, clip_fea=None, y=None):
         out = eng.forward("miss", self.cnt % 2)
         self.cnt = 0 if self.cnt + 1 >= self.num_steps else self.cnt + 1
         return [out]
-    ctypes, _lib, cfg, st = _tea_structs(self)
     slot = self.cnt % 2
     suffix = "even" if slot == 0 else "odd"
     e, e0 = eng.time_embedding()
-    modulated = (e0 if self.use_ref_steps else e).reshape(-1)  # :534
-    needs = ctypes.c_int32()
-    _lib.check(_lib.lib.mc_tea_needs_distance(ctypes.byref(cfg), ctypes.byref(st), ctypes.byref(needs)))
-    dist = ops.rel_l1(modulated, getattr(self, "previous_e0_" + suffix).reshape(-1)) if needs.value else 0.0
-    calc = ctypes.c_int32()
-    _lib.check(_lib.lib.mc_tea_decide(ctypes.byref(cfg), ctypes.byref(st), dist, ctypes.byref(calc)))
-    self.accumulated_rel_l1_distance_even, self.accumulated_rel_l1_distance_odd = st.accumulated[0], st.accumulated[1]
-    setattr(self, "previous_e0_" + suffix, modulated.clone().view((e0 if self.use_ref_steps else e).shape))  # :549 / :564
-    cur = getattr(self, "previous_residual_" + suffix)
-    if cur is None:
-        eng.res_valid[slot] = False
-    elif torch.is_tensor(cur) and cur.data_ptr() != eng.res[slot].data_ptr():
-        eng.res[slot].copy_(cur.reshape(eng.res[slot].shape))
-        eng.res_valid[slot] = True
+    emb = e0 if self.use_ref_steps else e
+    modulated = emb.reshape(-1)  # :534
+    calc = _TEA.decide(self, lambda: ops.rel_l1(modulated, getattr(self, "previous_e0_" + suffix).reshape(-1)))
+    setattr(self, "previous_e0_" + suffix, modulated.clone().view(emb.shape))  # :549 / :564
+    _take_residual(eng, getattr(self, "previous_residual_" + suffix), slot)
     eng.hit_sum_bf16 = True  # `x += self.previous_residual_*` in place on the bf16 patch embedding (:569 / :577): the sum is rounded to bf16
     try:
-        out = eng.forward("miss" if calc.value else "hit", slot)
+        out = eng.forward("miss" if calc else "hit", slot)
     finally:
         eng.hit_sum_bf16 = False
     setattr(self, "previous_residual_" + suffix, eng.res[slot].view(1, *eng.res[slot].shape))
-    _lib.check(_lib.lib.mc_tea_advance(ctypes.byref(cfg), ctypes.byref(st)))
-    self.cnt = st.cnt  # :587-589
+    _TEA.advance(self)  # :587-589
     return [out]
 
 

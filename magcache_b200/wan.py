@@ -551,6 +551,36 @@ class WanEngine:
             self.res_valid[slot] = True
         return out
 
+    def calibrate(self, slot, prev):
+        """The calibration forward (magcache_generate.py:80-194) for CFG slot `slot`: always runs the block stack; returns (head output,
+        (norm_ratio, norm_std, cos_dis) of the new residual against `prev`, or None when `prev` is None). The new residual is left in
+        `self.cal_residual` as a fresh fp32 [1, N, D] tensor (the reference rebinds `residual_cache[slot]` to it)."""
+        self._slot = slot
+        x0, e, e0, ctx = self.prologue()
+        xs = self.run_blocks(x0, e0, ctx, self.grid)
+        stats = None
+        if prev is None:
+            residual_x = ops.residual_sub(xs, x0)
+        else:
+            prev = prev.view(x0.shape)
+            reduce = None
+            if self.shard is not None:  # the statistics are sums over tokens: add the partial sums of every token shard
+                from .shard import allreduce_stats
+                reduce = lambda st: allreduce_stats(st, self.shard.group)  # noqa: E731
+            if self.pad_row:
+                # seq_len > token count: rows [n_tok, seq_len) of the reference's tensors are identical copies of the one pad row computed
+                # here; its three per-row terms enter the means (seq_len - n_tok) times (:167-169 average over dim 1 of [1, seq_len, D])
+                n_tok, wgt = self.n_keys, float(self.pad_weight)
+                keep = {}
+                ops.residual_sub_stats(xs[n_tok:], x0[n_tok:], prev[n_tok:].contiguous(), reduce=lambda st: keep.setdefault("pad", st.clone()))
+                residual_tok, stats = ops.residual_sub_stats(
+                    xs[:n_tok], x0[:n_tok], prev[:n_tok].contiguous(), reduce=lambda st: st + keep["pad"] * st.new_tensor([wgt, wgt, wgt, wgt]))
+                residual_x = torch.cat([residual_tok, xs[n_tok:] - x0[n_tok:].float()])
+            else:
+                residual_x, stats = ops.residual_sub_stats(xs, x0, prev, reduce=reduce)
+        self.cal_residual = residual_x.view(1, *x0.shape)
+        return self.head(xs, e, self.grid), stats
+
     # ------------------------------------------------------------------------------------------ block stack (:297-298)
     def run_blocks(self, x0, e0, ctx, grid):
         """30 (1.3B) / 40 (14B) WanAttentionBlocks (VACE models: the control-stream pass first, then the main blocks with their

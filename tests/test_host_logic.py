@@ -198,3 +198,17 @@ def test_handle_form_equals_the_struct_form(L):
     bad = _cfg(L, "wan2.1", [1.0] * 4, 4, 0.1, 2, 0.0)  # retention 0: the first call would hit an empty cache
     assert not L.lib.mc_ctrl_create(ctypes.byref(bad), 0) and b"mc_ctrl_validate" in L.lib.mc_last_error()
     L.lib.mc_ctrl_destroy(None)
+
+
+@pytest.mark.parametrize("attr", ["_mc_engine", "_mc_flux_engine", "_mc_hunyuan_engine", "_mc_opensora_engine"])
+def test_engine_cache_attrs(attr):
+    """Every engine kind a patched forward caches: `enable_token_shard` refuses to come after it, `invalidate_engine` drops it."""
+    import magcache_b200 as mc
+    m = type("M", (), {})()
+    m.__dict__[attr] = object()
+    m.__dict__["_mc_ctrls"] = {}
+    with pytest.raises(RuntimeError, match="before the first forward"):
+        mc.enable_token_shard(m, 0, 2)
+    mc.invalidate_engine(m)
+    assert attr not in m.__dict__ and "_mc_ctrls" not in m.__dict__
+    mc.enable_token_shard(m, 0, 2)

@@ -79,6 +79,8 @@ def _worker(rank, world, initfile, results, family):
                 for i in range(4):
                     call(m, i)
             cal[name] = [list(getattr(m, k)) for k in ("norm_ratio", "norm_std", "cos_dis")]
+            ceng = getattr(m, eng_attr)
+            cal[name + "_sharded"] = ceng.shard is not None and ceng.n_img * 2 == ceng.n_img_total
         results[rank] = (errs, res_err, eng.n_img, eng.n_img_total, eng.S_keys, cal)
     finally:
         dist.destroy_process_group()
@@ -94,6 +96,7 @@ def test_sharded_mmdit_engine_equals_single_world2(family):
         for r in (0, 1):
             errs, res_err, n_loc, n_tot, s_keys, cal = results[r]
             assert all(len(v) == 3 for v in cal["single"]) and all(len(v) == 3 for v in cal["sharded"]), cal
+            assert cal["sharded_sharded"] and not cal["single_sharded"]   # the calibration twin really ran on a token-sharded engine
             for a, b in zip(sum(cal["sharded"], []), sum(cal["single"], [])):
                 assert abs(a - b) <= 2e-2 * abs(b) + 2e-3, cal
             assert n_loc * 2 == n_tot == 48 and s_keys == 48 + (19 if family == "flux" else 11)

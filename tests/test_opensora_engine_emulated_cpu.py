@@ -10,6 +10,7 @@ import torch
 from magcache_b200 import opensora as os_mod
 from magcache_b200 import patch as patch_mod
 
+import magcache_b200 as mc
 import opensora_emu
 import opensora_ref as R
 
@@ -93,6 +94,45 @@ def test_replaced_residual_cache_is_read_at_last_index(emulated):
         r = ref(x, ts, None, y, **kw)
     assert ref.last_skip
     assert rel_l2(o, r) < 2e-2
+
+
+def test_invalidate_engine_repacks_changed_weights(emulated):
+    """After a weight change and `invalidate_engine`, the next forward runs on the new weights (the engine holds a packed copy)."""
+    ref, ref64, ours = _pair()
+    B, T, H, W = 2, 3, 6, 10
+    x, y, mask = _inputs(B, T, H, W, (12, 7))
+    kw = dict(mask=mask, fps=torch.tensor([24.0]), height=torch.tensor([8.0 * H]), width=torch.tensor([8.0 * W]))
+    ts = torch.tensor([1000.0, 990.0])
+
+    def run():
+        return ref(x, ts, None, y, **kw), ref64(x.double(), ts.to(torch.bfloat16).double(), None, y.double(), **kw), ours(x, ts, None, y, **kw)
+
+    with torch.no_grad():
+        run()
+        for m in (ref, ref64, ours):
+            for p in m.final_layer.parameters():
+                p.mul_(2.0)
+        mc.invalidate_engine(ours)
+        r, r64, o = run()
+    assert not ref.last_skip
+    e_ref = rel_l2(r, r64)
+    assert rel_l2(o, r64) <= 1.5 * e_ref + 1e-3, (rel_l2(o, r64), e_ref)
+
+
+def test_token_shard_rejected(emulated):
+    """The Open-Sora engine has no token-sharded path: a shard over more than one rank raises instead of having every rank compute
+    the whole video, and `enable_token_shard` after the first forward raises like for the other engines."""
+    _, _, ours = _pair()
+    x, y, mask = _inputs(1, 2, 4, 6, (9,))
+    kw = dict(mask=mask, fps=torch.tensor([24.0]), height=torch.tensor([32.0]), width=torch.tensor([48.0]))
+    mc.enable_token_shard(ours, 0, 2)
+    with pytest.raises(NotImplementedError, match="token sharding"), torch.no_grad():
+        ours(x, torch.tensor([900.0]), None, y, **kw)
+    _, _, ours = _pair()
+    with torch.no_grad():
+        ours(x, torch.tensor([900.0]), None, y, **kw)
+    with pytest.raises(RuntimeError, match="before the first forward"):
+        mc.enable_token_shard(ours, 0, 2)
 
 
 def test_unsupported_inputs_raise():
