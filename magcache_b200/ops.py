@@ -420,6 +420,7 @@ def attention(q, k, v, heads, scale=None, out=None, tag=None, first_key_row=0, s
         scale = 1.0 / math.sqrt(128)
     if out is None:
         out = torch.empty(Lq, W, dtype=torch.bfloat16, device=q.device)
+    assert out.dtype == torch.bfloat16 and out.stride(1) == 1 and out.shape == (Lq, W)
     need = ctypes.c_int64(0)
     check(lib.mc_attn_workspace_bytes(Lq, Lk, heads, ctypes.byref(need)))
     ws = _workspace("attention", q.device, need.value) if need.value > 0 else None

@@ -582,7 +582,8 @@ def _attn_ref(q, k, v, heads):
 
 
 @pytest.mark.parametrize("Lq,Lk,heads,qscale", [(128, 64, 1, 1.0), (128, 128, 1, 1.0), (256, 512, 2, 1.0), (300, 1000, 3, 1.0), (1000, 4095, 12, 1.0),
-                                                (200, 777, 2, 6.0), (130, 512, 12, 1.0)])
+                                                (200, 777, 2, 6.0), (130, 512, 12, 1.0),
+                                                (11, 11, 24, 1.0), (300, 65, 3, 1.0)])  # HunyuanVideo token refiner: Lk < 64 and Lq < 128
 def test_attention(Lq, Lk, heads, qscale):
     ops = _ops()
     W = heads * 128
