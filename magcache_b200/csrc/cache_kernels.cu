@@ -9,6 +9,7 @@
 
 #include "common.cuh"
 #include "ptx.cuh"
+#include "ring.cuh"
 
 namespace mc {
 
@@ -250,6 +251,33 @@ __global__ void __launch_bounds__(256) rel_l1_kernel(const float* __restrict__ c
 }
 
 // ---- K3: per-row norms / cosine, single pass ---------------------------------------------------------------
+// Lane partial sums of one row: cur^2, prev^2 and cur * prev over 8 elements
+__device__ __forceinline__ void stats_acc8(const float (&c)[8], const float (&p)[8], float& cc, float& pp, float& cp) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    cc = fmaf(c[j], c[j], cc);
+    pp = fmaf(p[j], p[j], pp);
+    cp = fmaf(c[j], p[j], cp);
+  }
+}
+
+// End of one row (whole warp): reduce the lane partial sums, then lane 0 adds the row's norm ratio, its square and its cosine
+// distance to acc[0..2] in double.
+__device__ __forceinline__ void stats_row(float cc, float pp, float cp, double denom_eps, int lane, double (&acc)[3]) {
+  cc = warp_sum(cc);
+  pp = warp_sum(pp);
+  cp = warp_sum(cp);
+  if (lane == 0) {
+    const float n_cur = sqrtf(cc), n_prev = sqrtf(pp);
+    const float ratio = n_cur / (n_prev + static_cast<float>(denom_eps));
+    // F.cosine_similarity(eps=1e-8): sum((a/max(|a|,eps)) * (b/max(|b|,eps)))
+    const float cosv = cp / (fmaxf(n_cur, 1e-8f) * fmaxf(n_prev, 1e-8f));
+    acc[0] += static_cast<double>(ratio);
+    acc[1] += static_cast<double>(ratio) * static_cast<double>(ratio);
+    acc[2] += static_cast<double>(1.0f - cosv);
+  }
+}
+
 // One warp per row; lanes stride over 8-element groups. Optionally also forms cur = xo - xi on the fly and stores it.
 template <int DCUR, int DPREV, bool FUSE_SUB>
 __global__ void __launch_bounds__(256) stats_kernel(const void* __restrict__ cur_or_xo, const void* __restrict__ xi_bf16,
@@ -257,7 +285,7 @@ __global__ void __launch_bounds__(256) stats_kernel(const void* __restrict__ cur
                                                     double denom_eps, double* __restrict__ stats) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps_per_block = blockDim.x >> 5;
   const int groups = cols >> 3;
-  double acc_ratio = 0.0, acc_ratio2 = 0.0, acc_cos = 0.0;
+  double acc[3] = {0.0, 0.0, 0.0};
   for (int64_t row = static_cast<int64_t>(blockIdx.x) * warps_per_block + warp; row < rows;
        row += static_cast<int64_t>(gridDim.x) * warps_per_block) {
     const int64_t base = row * cols;
@@ -285,33 +313,17 @@ __global__ void __launch_bounds__(256) stats_kernel(const void* __restrict__ cur
         const int g = g0 + 32 * u;
         if (g < groups) {
           if (FUSE_SUB) Elem<MC_F32>::store8(r_out, base + g * 8, c[u]);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            cc = fmaf(c[u][j], c[u][j], cc);
-            pp = fmaf(p[u][j], p[u][j], pp);
-            cp = fmaf(c[u][j], p[u][j], cp);
-          }
+          stats_acc8(c[u], p[u], cc, pp, cp);
         }
       }
     }
-    cc = warp_sum(cc);
-    pp = warp_sum(pp);
-    cp = warp_sum(cp);
-    if (lane == 0) {
-      const float n_cur = sqrtf(cc), n_prev = sqrtf(pp);
-      const float ratio = n_cur / (n_prev + static_cast<float>(denom_eps));
-      // F.cosine_similarity(eps=1e-8): sum((a/max(|a|,eps)) * (b/max(|b|,eps)))
-      const float cosv = cp / (fmaxf(n_cur, 1e-8f) * fmaxf(n_prev, 1e-8f));
-      acc_ratio += static_cast<double>(ratio);
-      acc_ratio2 += static_cast<double>(ratio) * static_cast<double>(ratio);
-      acc_cos += static_cast<double>(1.0f - cosv);
-    }
+    stats_row(cc, pp, cp, denom_eps, lane, acc);
   }
   __shared__ double sh[3][8];
   if (lane == 0) {
-    sh[0][warp] = acc_ratio;
-    sh[1][warp] = acc_ratio2;
-    sh[2][warp] = acc_cos;
+    sh[0][warp] = acc[0];
+    sh[1][warp] = acc[1];
+    sh[2][warp] = acc[2];
   }
   __syncthreads();
   if (threadIdx.x < 3) {
@@ -321,11 +333,12 @@ __global__ void __launch_bounds__(256) stats_kernel(const void* __restrict__ cur
   }
 }
 
-// TMA-staged variant for fp32 residuals (the Wan stream): a producer thread keeps kStages x (4 rows of each tensor) in flight
-// with cp.async.bulk into a shared-memory ring, so the bytes in flight per SM (~150 KB) no longer depend on how many warps
-// happen to be in their load phase; four consumer warps (one row each) reduce out of shared memory with warp shuffles.
-// Same arithmetic as stats_kernel. FUSE_SUB additionally stages x_in (bf16) and writes r = x_out - x_in.
+// TMA-staged variant for fp32 residuals (the Wan stream): the producer of a StageRing keeps kStages x (4 rows of each tensor) in
+// flight, so the bytes in flight per SM (~150 KB) no longer depend on how many warps happen to be in their load phase; four
+// consumer warps (one row each) reduce out of shared memory with warp shuffles. Same arithmetic as stats_kernel. FUSE_SUB
+// additionally stages x_in (bf16) and writes r = x_out - x_in.
 constexpr int kStatRows = 4;  // rows per stage = consumer warps
+constexpr int kStatMaxStages = 6;
 
 template <bool FUSE_SUB>
 __global__ void __launch_bounds__(160) stats_tma_kernel(const float* __restrict__ cur_or_xo, const __nv_bfloat16* __restrict__ xi,
@@ -333,53 +346,38 @@ __global__ void __launch_bounds__(160) stats_tma_kernel(const float* __restrict_
                                                         int stages, double denom_eps, double* __restrict__ stats) {
   extern __shared__ __align__(128) uint8_t smem_dyn[];
   const int row_f32 = cols * 4, row_bf16 = cols * 2;
-  const int stage_bytes = kStatRows * (2 * row_f32 + (FUSE_SUB ? row_bf16 : 0));
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem_dyn + static_cast<size_t>(stages) * stage_bytes);
-  uint64_t* empty = full + stages;
-  double* red = reinterpret_cast<double*>(empty + stages);  // [3][kStatRows]
+  const StageRing ring(smem_dyn, stages, kStatRows * (2 * row_f32 + (FUSE_SUB ? row_bf16 : 0)), kStatRows);
+  double* red = reinterpret_cast<double*>(ring.end());  // [3][kStatRows]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t n_chunks = (rows + kStatRows - 1) / kStatRows;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < stages; ++s) {
-      ptx::mbar_init(&full[s], 1);
-      ptx::mbar_init(&empty[s], kStatRows);
-    }
-    ptx::fence_mbar_init();
-  }
-  __syncthreads();
 
   if (warp == kStatRows) {
     // ---- producer warp (one thread): bulk copies of whole row groups, rows are contiguous in memory
     if (lane == 0) {
-      uint32_t it = 0;
-      for (int64_t c = blockIdx.x; c < n_chunks; c += gridDim.x, ++it) {
-        const int s = it % stages;
-        ptx::mbar_wait(&empty[s], ((it / stages) & 1) ^ 1);
-        const int64_t row0 = c * kStatRows;
-        const int64_t left = rows - row0;
-        const int nr = left < kStatRows ? static_cast<int>(left) : kStatRows;
-        uint8_t* base = smem_dyn + static_cast<size_t>(s) * stage_bytes;
-        const uint32_t bytes = static_cast<uint32_t>(nr) * (2 * row_f32 + (FUSE_SUB ? row_bf16 : 0));
-        ptx::mbar_expect_tx(&full[s], bytes);
-        ptx::bulk_load_1d(base, cur_or_xo + row0 * cols, nr * row_f32, &full[s]);
-        ptx::bulk_load_1d(base + kStatRows * row_f32, prev + row0 * cols, nr * row_f32, &full[s]);
-        if (FUSE_SUB) ptx::bulk_load_1d(base + 2 * kStatRows * row_f32, xi + row0 * cols, nr * row_bf16, &full[s]);
-      }
+      auto rows_in = [&](int64_t c) {
+        const int64_t left = rows - c * kStatRows;
+        return left < kStatRows ? static_cast<int>(left) : kStatRows;
+      };
+      ring.produce(
+          n_chunks, [&](int64_t c) { return static_cast<uint32_t>(rows_in(c)) * (2 * row_f32 + (FUSE_SUB ? row_bf16 : 0)); },
+          [&](int64_t c, uint8_t* slot, uint64_t* bar) {
+            const int64_t row0 = c * kStatRows;
+            const int nr = rows_in(c);
+            ptx::bulk_load_1d(slot, cur_or_xo + row0 * cols, nr * row_f32, bar);
+            ptx::bulk_load_1d(slot + kStatRows * row_f32, prev + row0 * cols, nr * row_f32, bar);
+            if (FUSE_SUB) ptx::bulk_load_1d(slot + 2 * kStatRows * row_f32, xi + row0 * cols, nr * row_bf16, bar);
+          });
     }
   } else {
     // ---- consumer warps: warp w owns row w of every stage
-    double acc_ratio = 0.0, acc_ratio2 = 0.0, acc_cos = 0.0;
+    double acc[3] = {0.0, 0.0, 0.0};
     const int groups = cols >> 3;
-    uint32_t it = 0;
-    for (int64_t c = blockIdx.x; c < n_chunks; c += gridDim.x, ++it) {
-      const int s = it % stages;
-      ptx::mbar_wait(&full[s], (it / stages) & 1);
+    ring.consume<1>(n_chunks, 0, [&](int64_t c, const uint8_t* stage, auto release) {
       const int64_t row = c * kStatRows + warp;
       if (row < rows) {
-        const uint8_t* base = smem_dyn + static_cast<size_t>(s) * stage_bytes;
-        const float4* cp4 = reinterpret_cast<const float4*>(base + warp * row_f32);
-        const float4* pp4 = reinterpret_cast<const float4*>(base + kStatRows * row_f32 + warp * row_f32);
-        const uint4* xp = reinterpret_cast<const uint4*>(base + 2 * kStatRows * row_f32 + warp * row_bf16);
+        const float4* cp4 = reinterpret_cast<const float4*>(stage + warp * row_f32);
+        const float4* pp4 = reinterpret_cast<const float4*>(stage + kStatRows * row_f32 + warp * row_f32);
+        const uint4* xp = reinterpret_cast<const uint4*>(stage + 2 * kStatRows * row_f32 + warp * row_bf16);
         float cc = 0.f, pp = 0.f, cp = 0.f;
         for (int g = lane; g < groups; g += 32) {
           float cv[8], pv[8];
@@ -393,32 +391,16 @@ __global__ void __launch_bounds__(160) stats_tma_kernel(const float* __restrict_
             for (int j = 0; j < 8; ++j) cv[j] = cv[j] - xv[j];
             Elem<MC_F32>::store8(r_out, row * cols + g * 8, cv);
           }
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            cc = fmaf(cv[j], cv[j], cc);
-            pp = fmaf(pv[j], pv[j], pp);
-            cp = fmaf(cv[j], pv[j], cp);
-          }
+          stats_acc8(cv, pv, cc, pp, cp);
         }
-        cc = warp_sum(cc);
-        pp = warp_sum(pp);
-        cp = warp_sum(cp);
-        if (lane == 0) {
-          const float n_cur = sqrtf(cc), n_prev = sqrtf(pp);
-          const float ratio = n_cur / (n_prev + static_cast<float>(denom_eps));
-          const float cosv = cp / (fmaxf(n_cur, 1e-8f) * fmaxf(n_prev, 1e-8f));
-          acc_ratio += static_cast<double>(ratio);
-          acc_ratio2 += static_cast<double>(ratio) * static_cast<double>(ratio);
-          acc_cos += static_cast<double>(1.0f - cosv);
-        }
+        stats_row(cc, pp, cp, denom_eps, lane, acc);
       }
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&empty[s]);  // this warp is done reading the stage
-    }
+      release();  // this warp is done reading the stage
+    });
     if (lane == 0) {
-      red[0 * kStatRows + warp] = acc_ratio;
-      red[1 * kStatRows + warp] = acc_ratio2;
-      red[2 * kStatRows + warp] = acc_cos;
+      red[0 * kStatRows + warp] = acc[0];
+      red[1 * kStatRows + warp] = acc[1];
+      red[2 * kStatRows + warp] = acc[2];
     }
   }
   __syncthreads();
@@ -442,23 +424,11 @@ static int32_t launch_stats(const void* cur, const void* xi, void* r_out, const 
   if (DCUR == MC_F32 && DPREV == MC_F32) {
     // TMA-staged path when at least two stages of 4 rows fit in shared memory (cols <= ~3000 for the plain statistics)
     const int stage_bytes = kStatRows * (2 * cols * 4 + (FUSE ? cols * 2 : 0));
-    int stages = (200 * 1024) / stage_bytes;
-    if (stages > 6) stages = 6;
-    if (stages >= 2) {
-      const int smem = stages * stage_bytes + stages * 16 + 3 * kStatRows * 8 + 64;
-      static bool attr_set = false;
-      if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(stats_tma_kernel<FUSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024);
-        if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(stats_tma smem)");
-        attr_set = true;
-      }
-      const int64_t n_chunks = (rows + kStatRows - 1) / kStatRows;
-      const int grid = static_cast<int>(n_chunks < num_sms() ? n_chunks : num_sms());
-      stats_tma_kernel<FUSE><<<grid, 160, smem, s>>>(static_cast<const float*>(cur), static_cast<const __nv_bfloat16*>(xi),
-                                                     static_cast<float*>(r_out), static_cast<const float*>(prev), rows, cols, stages, eps, stats);
-      MC_CHECK_LAUNCH("stats_tma_kernel launch");
-      return MC_OK;
-    }
+    const int stages = ring_stages(stage_bytes, kStatMaxStages);
+    if (stages > 0)
+      return launch_ring<stats_tma_kernel<FUSE>>(stages, stage_bytes, 3 * kStatRows * 8, (rows + kStatRows - 1) / kStatRows, (kStatRows + 1) * 32,
+                                                 s, "stats_tma_kernel", static_cast<const float*>(cur), static_cast<const __nv_bfloat16*>(xi),
+                                                 static_cast<float*>(r_out), static_cast<const float*>(prev), rows, cols, stages, eps, stats);
   }
   const int threads = 256, wpb = threads / 32;
   int64_t want = (rows + wpb - 1) / wpb;

@@ -56,9 +56,6 @@ inline int32_t set_max_smem_once(Kernel kernel, int bytes, PerDeviceOnce& once, 
 }
 
 // ---- device-side dtype helpers -----------------------------------------------------------------
-template <typename T>
-struct Vec8;  // 8 elements of T as one or two 128-bit words
-
 __device__ __forceinline__ float bf16_bits_to_f32(uint32_t hi16) { return __uint_as_float(hi16 << 16); }
 
 // unpack 8 bf16 (one uint4) to 8 floats
@@ -104,6 +101,17 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(u));
   const float hx = 0.5f * x;
   return fmaf(hx, t, hx);
+}
+
+// RoPE in fp32 on four consecutive (real, imag) pairs, cs holding (cos, sin) per pair: every product and every sum rounded on
+// its own (no FMA contraction), as torch computes `x * cos +- rotate(x) * sin` elementwise.
+__device__ __forceinline__ void rope_pairs4(float (&o)[8], const float (&cs)[8]) {
+#pragma unroll
+  for (int p = 0; p < 4; ++p) {
+    const float re = o[2 * p], im = o[2 * p + 1], c = cs[2 * p], sn = cs[2 * p + 1];
+    o[2 * p] = __fsub_rn(__fmul_rn(re, c), __fmul_rn(im, sn));
+    o[2 * p + 1] = __fadd_rn(__fmul_rn(re, sn), __fmul_rn(im, c));
+  }
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

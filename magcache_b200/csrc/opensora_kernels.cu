@@ -301,20 +301,18 @@ __global__ void __launch_bounds__(256) rmsnorm_head72_rope_kernel(__nv_bfloat16*
     const float r = rsqrtf(ss * (1.0f / os::kD) + eps);
 #pragma unroll
     for (int d = 0; d < os::kD; ++d) v[d] = round_bf16(round_bf16(v[d] * r) * __ldg(w + d));
-    if (cos_sin != nullptr) {
-      const float* cs = cos_sin + ((row / pos_div) % pos_mod) * os::kD;
-#pragma unroll
-      for (int i = 0; i < os::kD / 2; ++i) {
-        const float re = v[2 * i], im = v[2 * i + 1], c = __ldg(cs + 2 * i), sn = __ldg(cs + 2 * i + 1);
-        v[2 * i] = __fsub_rn(__fmul_rn(re, c), __fmul_rn(im, sn));
-        v[2 * i + 1] = __fadd_rn(__fmul_rn(im, c), __fmul_rn(re, sn));
-      }
-    }
+    const float* cs = cos_sin != nullptr ? cos_sin + ((row / pos_div) % pos_mod) * os::kD : nullptr;
 #pragma unroll
     for (int c = 0; c < 9; ++c) {
       float f[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) f[e] = v[c * 8 + e];
+      if (cs != nullptr) {
+        float cs8[8];
+#pragma unroll
+        for (int e = 0; e < 8; ++e) cs8[e] = __ldg(cs + c * 8 + e);
+        rope_pairs4(f, cs8);
+      }
       *reinterpret_cast<uint4*>(px + c * 8) = pack_bf16x8(f);
     }
   }

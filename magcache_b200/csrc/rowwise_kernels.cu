@@ -2,27 +2,29 @@
 // Arithmetic follows upstream Wan2.1 wan/modules/model.py as restated in SURVEY.md Appendix B.1; call sites in the
 // reference: MagCache4Wan2.1/magcache_generate.py:237 (patch_embedding), :249-254 (time embedding),
 // :297-298 (block stack), :304-305 (head, unpatchify).
+#include <type_traits>
+
 #include "common.cuh"
 #include "ptx.cuh"
+#include "ring.cuh"
 
 namespace mc {
 
-// A "team" of TPR threads owns one row; each thread keeps up to kMaxG groups of 8 elements in registers.
-// TPR = 32 (one warp per row, shuffle-only reductions) covers cols <= 2048; TPR = 128 covers cols <= 8192.
+// A row's 8-element groups are spread over the lanes that share the row, each lane keeping up to kMaxG groups in registers: one
+// warp per row covers cols <= 2048; the wide forms, a team of kWideWarps warps per row, cover cols <= 8192.
 constexpr int kMaxG = 8;
+constexpr int kWideWarps = 4;
 
-template <int TPR>
-__device__ __forceinline__ float team_sum(float v, float* scratch /* [rows_per_block][TPR/32] */, int team, int lane_in_team) {
+// sum over the kWideWarps warps of a team (scratch: [teams per block][kWideWarps])
+__device__ __forceinline__ float team_sum(float v, float* scratch, int team, int lane_in_team) {
   v = warp_sum(v);
-  if (TPR == 32) return v;
-  constexpr int W = TPR / 32;
   const int w = lane_in_team >> 5;
   __syncthreads();  // protect scratch reuse between consecutive reductions
-  if ((lane_in_team & 31) == 0) scratch[team * W + w] = v;
+  if ((lane_in_team & 31) == 0) scratch[team * kWideWarps + w] = v;
   __syncthreads();
   float t = 0.f;
 #pragma unroll
-  for (int i = 0; i < W; ++i) t += scratch[team * W + i];
+  for (int i = 0; i < kWideWarps; ++i) t += scratch[team * kWideWarps + i];
   return t;
 }
 
@@ -39,16 +41,77 @@ __device__ __forceinline__ void load_param8(const float* p, float (&f)[8]) {  //
   f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
 }
 
+// ---- per-row arithmetic: every launch form below calls these, so all forms give the same bits -------------------------------
+// LayerNorm statistics of a row held in registers. Group i of this lane is column group lane + i * lanes; groups at or past
+// `groups` are left out. `reduce` sums over the lanes of the row. Two passes: the mean, then the variance from the squared
+// deviations. Returns rsqrt(var + eps) and sets `mean`.
+template <int G, typename Reduce>
+__device__ __forceinline__ float ln_rstd(const float (&v)[G][8], int lane, int lanes, int groups, float inv_n, float eps, Reduce reduce,
+                                         float& mean) {
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < G; ++i)
+    if (lane + i * lanes < groups) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s += v[i][j];
+    }
+  mean = reduce(s) * inv_n;
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < G; ++i)
+    if (lane + i * lanes < groups) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float d = v[i][j] - mean;
+        q = fmaf(d, d, q);
+      }
+    }
+  return rsqrtf(reduce(q) * inv_n + eps);
+}
+
+// Output of modes 0 / 1 for 8 elements of a row: y = LN(x) * (1 + a) + b (mode 0) or LN(x) * a + b (mode 1), a and b the
+// per-column parameters at pa / pb, the LN value first rounded to bf16 when round_ln; stored at out + off as bf16 or fp32.
+__device__ __forceinline__ void ln_modulate_store8(const float (&v)[8], float mean, float rstd, const float* pa, const float* pb, int mode,
+                                                   int round_ln, void* out, int out_bf16, int64_t off) {
+  float a[8], b[8], o[8];
+  load_param8(pa, a);
+  load_param8(pb, b);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    float y = (v[j] - mean) * rstd;
+    if (round_ln) y = round_bf16(y);
+    const float aa = (mode == 0) ? 1.0f + a[j] : a[j];
+    o[j] = __fadd_rn(__fmul_rn(y, aa), b[j]);  // torch eager: separate mul and add, no FMA contraction
+  }
+  if (out_bf16) {
+    ptx::st_na_v4(static_cast<__nv_bfloat16*>(out) + off, pack_bf16x8(o));
+  } else {
+    ptx::st_na_v8_f32(static_cast<float*>(out) + off, o);
+  }
+}
+
+// WanRMSNorm of 8 elements given r = rsqrt(mean(x^2) + eps): _norm(x.float()).type_as(x) * weight, the weight at w
+__device__ __forceinline__ void rms_weight8(const float (&x)[8], float r, const float* w, float (&o)[8]) {
+  float wv[8];
+  load_param8(w, wv);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) o[j] = round_bf16(x[j] * r) * wv[j];
+}
+
+struct WarpReduce {  // the `reduce` of the warp-per-row forms
+  __device__ __forceinline__ float operator()(float v) const { return warp_sum(v); }
+};
+
 // ---- K7: LayerNorm (no affine) + modulation / affine, optional bf16 rounding of the LN output -----------------
 //   mode 0: y = LN(x) * (1 + p0[scale_idx]) + p0[shift_idx]   with p0 = e = modulation + e0, fp32 [k, cols]
 //   mode 1: y = LN(x) * p0 + p1                               (elementwise affine)
-template <int TPR>
+// Wide form (cols > 2048): a team of kWideWarps warps per row.
 __global__ void __launch_bounds__(256) ln_modulate_kernel(const void* __restrict__ x, int x_bf16, int64_t rows, int cols, float eps,
                                                           int mode, const float* __restrict__ p0, const float* __restrict__ p1,
                                                           int scale_idx, int shift_idx, int round_ln, void* __restrict__ out,
                                                           int out_bf16) {
-  constexpr int RPB = 256 / TPR;  // rows per block
-  __shared__ float scratch[RPB * (TPR / 32 > 0 ? TPR / 32 : 1)];
+  constexpr int TPR = 32 * kWideWarps, RPB = 256 / TPR;  // threads per row, rows per block
+  __shared__ float scratch[RPB * kWideWarps];
   const int team = threadIdx.x / TPR, lt = threadIdx.x % TPR;
   const int groups = cols >> 3;
   const float inv_n = 1.0f / static_cast<float>(cols);
@@ -56,54 +119,19 @@ __global__ void __launch_bounds__(256) ln_modulate_kernel(const void* __restrict
   const float* pb = (mode == 0) ? p0 + static_cast<int64_t>(shift_idx) * cols : p1;
   for (int64_t row0 = static_cast<int64_t>(blockIdx.x) * RPB; row0 < rows; row0 += static_cast<int64_t>(gridDim.x) * RPB) {
     const int64_t row = row0 + team;
-    const bool live = row < rows;
+    const int live_groups = row < rows ? groups : 0;  // a team past the last row still takes part in the block's reductions
     float v[kMaxG][8];
-    float s = 0.f;
 #pragma unroll
     for (int i = 0; i < kMaxG; ++i) {
       const int g = lt + i * TPR;
-      if (live && g < groups) {
-        load_row_group(x, x_bf16, row * cols + g * 8, v[i]);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) s += v[i][j];
-      }
+      if (g < live_groups) load_row_group(x, x_bf16, row * cols + g * 8, v[i]);
     }
-    const float mean = team_sum<TPR>(s, scratch, team, lt) * inv_n;
-    float q = 0.f;
+    float mean;
+    const float rstd = ln_rstd<kMaxG>(v, lt, TPR, live_groups, inv_n, eps, [&](float t) { return team_sum(t, scratch, team, lt); }, mean);
 #pragma unroll
     for (int i = 0; i < kMaxG; ++i) {
       const int g = lt + i * TPR;
-      if (live && g < groups) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float d = v[i][j] - mean;
-          q = fmaf(d, d, q);
-        }
-      }
-    }
-    const float var = team_sum<TPR>(q, scratch, team, lt) * inv_n;
-    const float rstd = rsqrtf(var + eps);
-#pragma unroll
-    for (int i = 0; i < kMaxG; ++i) {
-      const int g = lt + i * TPR;
-      if (live && g < groups) {
-        const int c0 = g * 8;
-        float a[8], b[8], o[8];
-        load_param8(pa + c0, a);
-        load_param8(pb + c0, b);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float y = (v[i][j] - mean) * rstd;
-          if (round_ln) y = round_bf16(y);
-          const float aa = (mode == 0) ? 1.0f + a[j] : a[j];
-          o[j] = __fadd_rn(__fmul_rn(y, aa), b[j]);  // torch eager: separate mul and add, no FMA contraction
-        }
-        if (out_bf16) {
-          ptx::st_na_v4(static_cast<__nv_bfloat16*>(out) + row * cols + c0, pack_bf16x8(o));
-        } else {
-          ptx::st_na_v8_f32(static_cast<float*>(out) + row * cols + c0, o);
-        }
-      }
+      if (g < live_groups) ln_modulate_store8(v[i], mean, rstd, pa + g * 8, pb + g * 8, mode, round_ln, out, out_bf16, row * cols + g * 8);
     }
   }
 }
@@ -120,29 +148,13 @@ __global__ void __launch_bounds__(256) ln_t2i_modulate_kernel(const __nv_bfloat1
   for (int64_t row = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; row < rows;
        row += (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5) {
     float v[kMaxG][8];
-    float s = 0.f;
 #pragma unroll
     for (int i = 0; i < kMaxG; ++i) {
       const int g = lane + i * 32;
-      if (g < groups) {
-        unpack_bf16x8(ptx::ld_nc_v4(x + row * cols + g * 8), v[i]);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) s += v[i][j];
-      }
+      if (g < groups) unpack_bf16x8(ptx::ld_nc_v4(x + row * cols + g * 8), v[i]);
     }
-    const float mean = warp_sum(s) * inv_n;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < kMaxG; ++i) {
-      if (lane + i * 32 < groups) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float d = v[i][j] - mean;
-          q = fmaf(d, d, q);
-        }
-      }
-    }
-    const float rstd = rsqrtf(warp_sum(q) * inv_n + eps);
+    float mean;
+    const float rstd = ln_rstd<kMaxG>(v, lane, 32, groups, inv_n, eps, WarpReduce(), mean);
 #pragma unroll
     for (int i = 0; i < kMaxG; ++i) {
       const int g = lane + i * 32;
@@ -162,12 +174,12 @@ __global__ void __launch_bounds__(256) ln_t2i_modulate_kernel(const __nv_bfloat1
 }
 
 // ---- WanRMSNorm over the model dim (+ optional 3-axis RoPE), in place on bf16 ---------------------------------
-template <int TPR>
+// Wide form (cols > 2048): a team of kWideWarps warps per row.
 __global__ void __launch_bounds__(256) rmsnorm_rope_kernel(__nv_bfloat16* __restrict__ x, int64_t ld, int64_t rows, int cols,
                                                            const float* __restrict__ w, float eps,
                                                            const float* __restrict__ cos_sin, int head_dim) {
-  constexpr int RPB = 256 / TPR;
-  __shared__ float scratch[RPB * (TPR / 32 > 0 ? TPR / 32 : 1)];
+  constexpr int TPR = 32 * kWideWarps, RPB = 256 / TPR;
+  __shared__ float scratch[RPB * kWideWarps];
   const int team = threadIdx.x / TPR, lt = threadIdx.x % TPR;
   const int groups = cols >> 3;
   const float inv_n = 1.0f / static_cast<float>(cols);
@@ -186,27 +198,18 @@ __global__ void __launch_bounds__(256) rmsnorm_rope_kernel(__nv_bfloat16* __rest
         for (int j = 0; j < 8; ++j) q = fmaf(v[i][j], v[i][j], q);
       }
     }
-    const float ms = team_sum<TPR>(q, scratch, team, lt) * inv_n;
-    const float r = rsqrtf(ms + eps);
+    const float r = rsqrtf(team_sum(q, scratch, team, lt) * inv_n + eps);
 #pragma unroll
     for (int i = 0; i < kMaxG; ++i) {
       const int g = lt + i * TPR;
       if (live && g < groups) {
         const int c0 = g * 8;
-        float wv[8], o[8];
-        load_param8(w + c0, wv);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = round_bf16(v[i][j] * r) * wv[j];  // _norm(x.float()).type_as(x) * weight
+        float o[8];
+        rms_weight8(v[i], r, w + c0, o);
         if (cos_sin != nullptr) {
-          const int d0 = c0 % head_dim;  // position inside the head; 8 elements = 4 complex pairs
           float cs[8];
-          ptx::ld_nc_v8_f32(cos_sin + row * head_dim + d0, cs);
-#pragma unroll
-          for (int p = 0; p < 4; ++p) {
-            const float re = o[2 * p], im = o[2 * p + 1], c = cs[2 * p], sn = cs[2 * p + 1];
-            o[2 * p] = __fsub_rn(__fmul_rn(re, c), __fmul_rn(im, sn));
-            o[2 * p + 1] = __fadd_rn(__fmul_rn(re, sn), __fmul_rn(im, c));
-          }
+          ptx::ld_nc_v8_f32(cos_sin + row * head_dim + c0 % head_dim, cs);  // position inside the head; 8 elements = 4 pairs
+          rope_pairs4(o, cs);
         }
         *reinterpret_cast<uint4*>(x + row * ld + c0) = pack_bf16x8(o);
       }
@@ -238,46 +241,12 @@ __global__ void __launch_bounds__(256, (G >= 6 ? 1 : 2)) ln_modulate_pipe_kernel
     }
   };
   auto process = [&](int64_t row, float (&v)[G][8]) {
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < G; ++i)
-      if (lane + i * 32 < groups) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) s += v[i][j];
-      }
-    const float mean = warp_sum(s) * inv_n;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < G; ++i)
-      if (lane + i * 32 < groups) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float d = v[i][j] - mean;
-          q = fmaf(d, d, q);
-        }
-      }
-    const float rstd = rsqrtf(warp_sum(q) * inv_n + eps);
+    float mean;
+    const float rstd = ln_rstd<G>(v, lane, 32, groups, inv_n, eps, WarpReduce(), mean);
 #pragma unroll
     for (int i = 0; i < G; ++i) {
-      const int g = lane + i * 32;
-      if (g < groups) {
-        const int c0 = g * 8;
-        float a[8], b[8], o[8];
-        load_param8(pa + c0, a);
-        load_param8(pb + c0, b);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float y = (v[i][j] - mean) * rstd;
-          if (round_ln) y = round_bf16(y);
-          const float aa = (mode == 0) ? 1.0f + a[j] : a[j];
-          o[j] = __fadd_rn(__fmul_rn(y, aa), b[j]);  // torch eager: separate mul and add, no FMA contraction
-        }
-        if (out_bf16) {
-          ptx::st_na_v4(static_cast<__nv_bfloat16*>(out) + row * cols + c0, pack_bf16x8(o));
-        } else {
-          ptx::st_na_v8_f32(static_cast<float*>(out) + row * cols + c0, o);
-        }
-      }
+      const int c0 = (lane + i * 32) * 8;
+      if (c0 < cols) ln_modulate_store8(v[i], mean, rstd, pa + c0, pb + c0, mode, round_ln, out, out_bf16, row * cols + c0);
     }
   };
   float va[G][8], vb[G][8];
@@ -335,21 +304,13 @@ __global__ void __launch_bounds__(256, 2) rmsnorm_rope_pipe_kernel(__nv_bfloat16
       const int g = lane + i * 32;
       if (g < groups) {
         const int c0 = g * 8;
-        float f[8], wv[8], o[8];
+        float f[8], o[8];
         unpack_bf16x8(raw[i], f);
-        load_param8(ws + c0, wv);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = round_bf16(f[j] * r) * wv[j];  // _norm(x.float()).type_as(x) * weight
+        rms_weight8(f, r, ws + c0, o);
         if (cos_sin != nullptr) {
-          const int d0 = c0 % head_dim;  // position inside the head; 8 elements = 4 complex pairs
           float cs[8];
-          ptx::ld_nc_v8_f32(cos_sin + row * head_dim + d0, cs);
-#pragma unroll
-          for (int pp = 0; pp < 4; ++pp) {
-            const float re = o[2 * pp], im = o[2 * pp + 1], c = cs[2 * pp], sn = cs[2 * pp + 1];
-            o[2 * pp] = __fsub_rn(__fmul_rn(re, c), __fmul_rn(im, sn));
-            o[2 * pp + 1] = __fadd_rn(__fmul_rn(re, sn), __fmul_rn(im, c));
-          }
+          ptx::ld_nc_v8_f32(cos_sin + row * head_dim + c0 % head_dim, cs);  // position inside the head; 8 elements = 4 pairs
+          rope_pairs4(o, cs);
         }
         *reinterpret_cast<uint4*>(px + c0) = pack_bf16x8(o);
       }
@@ -371,15 +332,15 @@ __global__ void __launch_bounds__(256, 2) rmsnorm_rope_pipe_kernel(__nv_bfloat16
 
 // ---- TMA-staged forms of the same two kernels: the register-pipelined forms above keep one row per warp in flight (48-96 KB
 // per SM), which is short of the ~60 KB x latency a 6.5 TB/s stream needs once the warps also reduce, compute and store
-// (3.2-3.9 TB/s measured on 32760 x 1536). Here one producer thread keeps `stages` x 8 rows in flight with cp.async.bulk into a
-// shared-memory ring (144-192 KB per SM, independent of what the consumer warps are doing); NG groups of eight consumer warps
-// take the stages in turn (stage `it` belongs to group it % NG), one row of the stage per warp: copy it to registers, hand the
-// slot back at once, then run the same arithmetic as the forms above (bit-identical results). One CTA per SM, chunks of 8 rows
-// strided over the grid. The consumers, not the loads, bound these kernels: 8 warps 4.2 TB/s, 16 warps 4.7 TB/s on fp32 rows
-// (24 warps spill at 80 registers); the bf16 RMSNorm rows take 24 warps: 3.2 -> 5.1 TB/s.
+// (3.2-3.9 TB/s measured on 32760 x 1536). Here the producer of a StageRing keeps `stages` x 8 rows in flight (144-192 KB per
+// SM); NG groups of eight consumer warps take the stages in turn, one row of the stage per warp: copy it to registers, hand the
+// slot back at once, then run the same arithmetic as the forms above. One CTA per SM, chunks of 8 rows strided over the grid.
+// The consumers, not the loads, bound these kernels: 8 warps 4.2 TB/s, 16 warps 4.7 TB/s on fp32 rows (24 warps spill at 80
+// registers); the bf16 RMSNorm rows take 24 warps: 3.2 -> 5.1 TB/s.
 constexpr int kRingRows = 8;                                                   // rows (or (token, block) items) per stage
 constexpr int ring_threads(int groups) { return (groups * kRingRows + 1) * 32; }  // + the producer warp
 constexpr int kLnRingGroups = 2, kRmsRingGroups = 3;
+constexpr int kRowRingMaxStages = 8;
 
 template <int G, int NG>
 __global__ void __launch_bounds__(ring_threads(NG), 1) ln_modulate_tma_kernel(const void* __restrict__ x, int x_bf16, int64_t rows, int cols, float eps,
@@ -388,32 +349,19 @@ __global__ void __launch_bounds__(ring_threads(NG), 1) ln_modulate_tma_kernel(co
                                                                          int out_bf16, int stages) {
   extern __shared__ __align__(128) uint8_t smem_dyn[];
   const int row_bytes = cols * (x_bf16 ? 2 : 4);
-  const int stage_bytes = kRingRows * row_bytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem_dyn + static_cast<size_t>(stages) * stage_bytes);
-  uint64_t* empty = full + stages;
+  const StageRing ring(smem_dyn, stages, kRingRows * row_bytes, kRingRows);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t n_chunks = (rows + kRingRows - 1) / kRingRows;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < stages; ++s) {
-      ptx::mbar_init(&full[s], 1);
-      ptx::mbar_init(&empty[s], kRingRows);
-    }
-    ptx::fence_mbar_init();
-  }
-  __syncthreads();
 
   if (warp == NG * kRingRows) {
     if (lane == 0) {
-      uint32_t it = 0;
-      for (int64_t c = blockIdx.x; c < n_chunks; c += gridDim.x, ++it) {
-        const int s = it % stages;
-        ptx::mbar_wait(&empty[s], ((it / stages) & 1) ^ 1);
-        const int64_t row0 = c * kRingRows;
-        const int64_t left = rows - row0;
-        const uint32_t bytes = static_cast<uint32_t>(left < kRingRows ? left : kRingRows) * row_bytes;  // rows are contiguous
-        ptx::mbar_expect_tx(&full[s], bytes);
-        ptx::bulk_load_1d(smem_dyn + static_cast<size_t>(s) * stage_bytes, static_cast<const uint8_t*>(x) + row0 * row_bytes, bytes, &full[s]);
-      }
+      auto bytes = [&](int64_t c) {
+        const int64_t left = rows - c * kRingRows;
+        return static_cast<uint32_t>(left < kRingRows ? left : kRingRows) * row_bytes;
+      };
+      ring.produce(n_chunks, bytes, [&](int64_t c, uint8_t* slot, uint64_t* bar) {  // rows are contiguous: one copy
+        ptx::bulk_load_1d(slot, static_cast<const uint8_t*>(x) + c * kRingRows * row_bytes, bytes(c), bar);
+      });
     }
     return;
   }
@@ -423,12 +371,9 @@ __global__ void __launch_bounds__(ring_threads(NG), 1) ln_modulate_tma_kernel(co
   const float* pa = (mode == 0) ? p0 + static_cast<int64_t>(scale_idx) * cols : p0;
   const float* pb = (mode == 0) ? p0 + static_cast<int64_t>(shift_idx) * cols : p1;
   const int grp = warp / kRingRows, wr = warp - grp * kRingRows;  // consumer group, row of the stage
-  uint32_t it = grp;
-  for (int64_t c = blockIdx.x + static_cast<int64_t>(grp) * gridDim.x; c < n_chunks; c += static_cast<int64_t>(NG) * gridDim.x, it += NG) {
-    const int s = it % stages;
-    ptx::mbar_wait(&full[s], (it / stages) & 1);
+  ring.consume<NG>(n_chunks, grp, [&](int64_t c, const uint8_t* stage, auto release) {
     const int64_t row = c * kRingRows + wr;
-    const uint8_t* rp = smem_dyn + static_cast<size_t>(s) * stage_bytes + wr * row_bytes;
+    const uint8_t* rp = stage + wr * row_bytes;
     float v[G][8];
     if (row < rows) {
 #pragma unroll
@@ -444,51 +389,16 @@ __global__ void __launch_bounds__(ring_threads(NG), 1) ln_modulate_tma_kernel(co
         }
       }
     }
-    __syncwarp();
-    if (lane == 0) ptx::mbar_arrive(&empty[s]);  // the row is in registers: the slot can be refilled while it is processed
-    if (row >= rows) continue;
-    float sum = 0.f;
-#pragma unroll
-    for (int i = 0; i < G; ++i)
-      if (lane + i * 32 < groups) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) sum += v[i][j];
-      }
-    const float mean = warp_sum(sum) * inv_n;
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < G; ++i)
-      if (lane + i * 32 < groups) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float d = v[i][j] - mean;
-          q = fmaf(d, d, q);
-        }
-      }
-    const float rstd = rsqrtf(warp_sum(q) * inv_n + eps);
+    release();  // the row is in registers: the slot can be refilled while it is processed
+    if (row >= rows) return;
+    float mean;
+    const float rstd = ln_rstd<G>(v, lane, 32, groups, inv_n, eps, WarpReduce(), mean);
 #pragma unroll
     for (int i = 0; i < G; ++i) {
       const int g = lane + i * 32;
-      if (g < groups) {
-        const int c0 = g * 8;
-        float a[8], b[8], o[8];
-        load_param8(pa + c0, a);
-        load_param8(pb + c0, b);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float y = (v[i][j] - mean) * rstd;
-          if (round_ln) y = round_bf16(y);
-          const float aa = (mode == 0) ? 1.0f + a[j] : a[j];
-          o[j] = __fadd_rn(__fmul_rn(y, aa), b[j]);  // torch eager: separate mul and add, no FMA contraction
-        }
-        if (out_bf16) {
-          ptx::st_na_v4(static_cast<__nv_bfloat16*>(out) + row * cols + c0, pack_bf16x8(o));
-        } else {
-          ptx::st_na_v8_f32(static_cast<float*>(out) + row * cols + c0, o);
-        }
-      }
+      if (g < groups) ln_modulate_store8(v[i], mean, rstd, pa + g * 8, pb + g * 8, mode, round_ln, out, out_bf16, row * cols + g * 8);
     }
-  }
+  });
 }
 
 // items = (token, block); the `segs` blocks of a token are adjacent in memory, so a stage of 8 items is 8 / segs pitched rows of
@@ -501,35 +411,25 @@ __global__ void __launch_bounds__(ring_threads(NG), 1) rmsnorm_rope_tma_kernel(_
   const int item_bytes = cols * 2;
   const int rows_per_stage = kRingRows / segs;  // segs in {1, 2, 4}
   const int cs_row_bytes = cos_sin != nullptr ? head_dim * 4 : 0;
-  const int stage_bytes = kRingRows * item_bytes + rows_per_stage * cs_row_bytes;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem_dyn + static_cast<size_t>(stages) * stage_bytes);
-  uint64_t* empty = full + stages;
+  const StageRing ring(smem_dyn, stages, kRingRows * item_bytes + rows_per_stage * cs_row_bytes, kRingRows);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t n_chunks = (rows + rows_per_stage - 1) / rows_per_stage;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < stages; ++s) {
-      ptx::mbar_init(&full[s], 1);
-      ptx::mbar_init(&empty[s], kRingRows);
-    }
-    ptx::fence_mbar_init();
-  }
-  __syncthreads();
 
   if (warp == NG * kRingRows) {
     if (lane == 0) {
-      uint32_t it = 0;
-      for (int64_t c = blockIdx.x; c < n_chunks; c += gridDim.x, ++it) {
-        const int s = it % stages;
-        ptx::mbar_wait(&empty[s], ((it / stages) & 1) ^ 1);
-        const int64_t row0 = c * rows_per_stage;
-        const int64_t left = rows - row0;
-        const int nr = left < rows_per_stage ? static_cast<int>(left) : rows_per_stage;
-        uint8_t* base = smem_dyn + static_cast<size_t>(s) * stage_bytes;
-        const uint32_t per_row = static_cast<uint32_t>(segs) * item_bytes;
-        ptx::mbar_expect_tx(&full[s], static_cast<uint32_t>(nr) * (per_row + cs_row_bytes));
-        for (int r = 0; r < nr; ++r) ptx::bulk_load_1d(base + r * per_row, x + (row0 + r) * ld, per_row, &full[s]);
-        if (cs_row_bytes) ptx::bulk_load_1d(base + kRingRows * item_bytes, cos_sin + row0 * head_dim, nr * cs_row_bytes, &full[s]);
-      }
+      const uint32_t per_row = static_cast<uint32_t>(segs) * item_bytes;
+      auto rows_in = [&](int64_t c) {
+        const int64_t left = rows - c * rows_per_stage;
+        return left < rows_per_stage ? static_cast<int>(left) : rows_per_stage;
+      };
+      ring.produce(
+          n_chunks, [&](int64_t c) { return static_cast<uint32_t>(rows_in(c)) * (per_row + cs_row_bytes); },
+          [&](int64_t c, uint8_t* slot, uint64_t* bar) {
+            const int64_t row0 = c * rows_per_stage;
+            const int nr = rows_in(c);
+            for (int r = 0; r < nr; ++r) ptx::bulk_load_1d(slot + r * per_row, x + (row0 + r) * ld, per_row, bar);
+            if (cs_row_bytes) ptx::bulk_load_1d(slot + kRingRows * item_bytes, cos_sin + row0 * head_dim, nr * cs_row_bytes, bar);
+          });
     }
     return;
   }
@@ -539,13 +439,9 @@ __global__ void __launch_bounds__(ring_threads(NG), 1) rmsnorm_rope_tma_kernel(_
   const int grp = warp / kRingRows, wr = warp - grp * kRingRows;  // consumer group, item of the stage
   const int r_in_stage = wr / segs, seg = wr - r_in_stage * segs;
   const float* ws = w + static_cast<int64_t>(seg) * cols;
-  uint32_t it = grp;
-  for (int64_t c = blockIdx.x + static_cast<int64_t>(grp) * gridDim.x; c < n_chunks; c += static_cast<int64_t>(NG) * gridDim.x, it += NG) {
-    const int s = it % stages;
-    ptx::mbar_wait(&full[s], (it / stages) & 1);
+  ring.consume<NG>(n_chunks, grp, [&](int64_t c, const uint8_t* stage, auto release) {
     const int64_t row = c * rows_per_stage + r_in_stage;
-    const uint8_t* base = smem_dyn + static_cast<size_t>(s) * stage_bytes;
-    const uint8_t* rp = base + wr * item_bytes;  // item wr of the stage = (row r_in_stage, block seg)
+    const uint8_t* rp = stage + wr * item_bytes;  // item wr of the stage = (row r_in_stage, block seg)
     uint4 raw[G];
     float cs[8] = {1.f, 0.f, 1.f, 0.f, 1.f, 0.f, 1.f, 0.f};
     if (row < rows) {
@@ -556,14 +452,13 @@ __global__ void __launch_bounds__(ring_threads(NG), 1) rmsnorm_rope_tma_kernel(_
       }
       if (cs_row_bytes) {
         // a lane's groups are 256 columns apart: with head_dim dividing 256 they all sit at the same position inside their head
-        const float4* cp = reinterpret_cast<const float4*>(base + kRingRows * item_bytes + r_in_stage * cs_row_bytes + ((lane * 8) % head_dim) * 4);
+        const float4* cp = reinterpret_cast<const float4*>(stage + kRingRows * item_bytes + r_in_stage * cs_row_bytes + ((lane * 8) % head_dim) * 4);
         const float4 a = cp[0], b = cp[1];
         cs[0] = a.x; cs[1] = a.y; cs[2] = a.z; cs[3] = a.w; cs[4] = b.x; cs[5] = b.y; cs[6] = b.z; cs[7] = b.w;
       }
     }
-    __syncwarp();
-    if (lane == 0) ptx::mbar_arrive(&empty[s]);
-    if (row >= rows) continue;
+    release();
+    if (row >= rows) return;
     __nv_bfloat16* px = x + row * ld + static_cast<int64_t>(seg) * cols;
     float q = 0.f;
 #pragma unroll
@@ -580,30 +475,14 @@ __global__ void __launch_bounds__(ring_threads(NG), 1) rmsnorm_rope_tma_kernel(_
       const int g = lane + i * 32;
       if (g < groups) {
         const int c0 = g * 8;
-        float f[8], wv[8], o[8];
+        float f[8], o[8];
         unpack_bf16x8(raw[i], f);
-        load_param8(ws + c0, wv);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o[j] = round_bf16(f[j] * r) * wv[j];  // _norm(x.float()).type_as(x) * weight
-        if (cs_row_bytes) {
-#pragma unroll
-          for (int pp = 0; pp < 4; ++pp) {
-            const float re = o[2 * pp], im = o[2 * pp + 1], cc = cs[2 * pp], sn = cs[2 * pp + 1];
-            o[2 * pp] = __fsub_rn(__fmul_rn(re, cc), __fmul_rn(im, sn));
-            o[2 * pp + 1] = __fadd_rn(__fmul_rn(re, sn), __fmul_rn(im, cc));
-          }
-        }
+        rms_weight8(f, r, ws + c0, o);
+        if (cs_row_bytes) rope_pairs4(o, cs);
         *reinterpret_cast<uint4*>(px + c0) = pack_bf16x8(o);
       }
     }
-  }
-}
-
-// number of ring stages that fit (0: the staged form does not apply)
-static int ring_stages(int stage_bytes) {
-  int stages = (200 * 1024) / stage_bytes;
-  if (stages > 8) stages = 8;
-  return stages >= 2 ? stages : 0;
+  });
 }
 
 // ---- per-HEAD RMSNorm (head_dim 128, bf16 weight semantics) + RoPE, in place on bf16: the q / k normalisation of the MMDiT
@@ -640,12 +519,7 @@ __global__ void __launch_bounds__(256) rmsnorm_head_rope_kernel(__nv_bfloat16* _
     if (cos_sin != nullptr) {
       float cs[8];
       ptx::ld_nc_v8_f32(cos_sin + row * 128 + sub * 8, cs);
-#pragma unroll
-      for (int p = 0; p < 4; ++p) {
-        const float re = o[2 * p], im = o[2 * p + 1], c = cs[2 * p], sn = cs[2 * p + 1];
-        o[2 * p] = __fsub_rn(__fmul_rn(re, c), __fmul_rn(im, sn));
-        o[2 * p + 1] = __fadd_rn(__fmul_rn(im, c), __fmul_rn(re, sn));
-      }
+      rope_pairs4(o, cs);
     }
     *reinterpret_cast<uint4*>(px) = pack_bf16x8(o);
   }
@@ -694,8 +568,6 @@ __global__ void patchify_kernel(const float* __restrict__ lat, int C, int F, int
 }
 
 // ---- small fp32 linear (M <= 8): one warp per output feature -------------------------------------------------
-__device__ __forceinline__ float silu(float x) { return x / (1.0f + expf(-x)); }
-
 template <int M>
 __global__ void __launch_bounds__(256) linear_f32_small_kernel(const float* __restrict__ x, int K, const float* __restrict__ Wt,
                                                                const float* __restrict__ b, int N, int act, float* __restrict__ y) {
@@ -712,7 +584,7 @@ __global__ void __launch_bounds__(256) linear_f32_small_kernel(const float* __re
     for (int m = 0; m < M; ++m) {
       float4 xv = reinterpret_cast<const float4*>(x + static_cast<int64_t>(m) * K)[k4];
       if (act == 1) {
-        xv.x = silu(xv.x); xv.y = silu(xv.y); xv.z = silu(xv.z); xv.w = silu(xv.w);
+        xv.x = silu_f(xv.x); xv.y = silu_f(xv.y); xv.z = silu_f(xv.z); xv.w = silu_f(xv.w);
       }
       acc[m] = fmaf(xv.x, wv.x, acc[m]);
       acc[m] = fmaf(xv.y, wv.y, acc[m]);
@@ -725,7 +597,7 @@ __global__ void __launch_bounds__(256) linear_f32_small_kernel(const float* __re
     float t = warp_sum(acc[m]);
     if (lane == 0) {
       t += (b != nullptr) ? b[n] : 0.f;
-      if (act == 2) t = silu(t);
+      if (act == 2) t = silu_f(t);
       y[static_cast<int64_t>(m) * N + n] = t;
     }
   }
@@ -790,6 +662,16 @@ static int grid_for(int64_t work_items, int per_block) {
   return static_cast<int>(want < cap ? want : cap);
 }
 
+// f(std::integral_constant<int, G>{}) for the smallest G in {2, 4, 6, 8} with 32 lanes x G groups >= `groups` (groups <= 32 * kMaxG):
+// the per-lane register arrays the warp-per-row kernels are instantiated with
+template <typename F>
+static auto with_lane_groups(int groups, F f) {
+  if (groups <= 32 * 2) return f(std::integral_constant<int, 2>{});
+  if (groups <= 32 * 4) return f(std::integral_constant<int, 4>{});
+  if (groups <= 32 * 6) return f(std::integral_constant<int, 6>{});
+  return f(std::integral_constant<int, 8>{});
+}
+
 }  // namespace mc
 
 extern "C" {
@@ -822,51 +704,33 @@ int32_t mc_ln_modulate(const void* x, int32_t x_dtype, int64_t rows, int32_t col
     MC_CHECK_LAUNCH("ln_t2i_modulate_kernel launch");
     return MC_OK;
   }
-  MC_CHECK_ARG(rows >= 1 && cols >= 8 && cols % 8 == 0 && cols <= 128 * 8 * mc::kMaxG, "mc_ln_modulate: cols=%d unsupported", cols);
+  MC_CHECK_ARG(rows >= 1 && cols >= 8 && cols % 8 == 0 && cols <= 32 * mc::kWideWarps * 8 * mc::kMaxG, "mc_ln_modulate: cols=%d unsupported", cols);
   MC_CHECK_ARG(mc::aligned16(p0) && (p1 == nullptr || mc::aligned16(p1)), "mc_ln_modulate: parameters must be 16-byte aligned");
   MC_CHECK_ARG((x_dtype == MC_F32 || x_dtype == MC_BF16) && (out_dtype == MC_F32 || out_dtype == MC_BF16), "mc_ln_modulate: bad dtype");
   MC_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 31u) == 0 && (reinterpret_cast<uintptr_t>(out) & 31u) == 0,
                "mc_ln_modulate: x/out must be 32-byte aligned");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int groups = cols / 8;
-#define MC_LN(TPR)                                                                                                             \
-  mc::ln_modulate_kernel<TPR><<<mc::grid_for(rows, 256 / TPR), 256, 0, s>>>(x, x_dtype == MC_BF16, rows, cols, eps, mode,       \
-                                                                            p0, p1, scale_idx, shift_idx,                      \
-                                                                            round_ln_to_bf16, out, out_dtype == MC_BF16)
-#define MC_LNP(G)                                                                                                              \
-  mc::ln_modulate_pipe_kernel<G><<<mc::pipe_grid(rows, (G) >= 6 ? 1 : 2), 256, 0, s>>>(x, x_dtype == MC_BF16, rows, cols, eps, mode, p0, p1,      \
-                                                                     scale_idx, shift_idx, round_ln_to_bf16, out, out_dtype == MC_BF16)
+  const int x_bf16 = x_dtype == MC_BF16, o_bf16 = out_dtype == MC_BF16;
   // long inputs: the TMA-staged form (needs >= 2 stages of 8 rows in shared memory and 16-byte aligned rows)
-  const int ring = rows >= 1024 && groups <= 32 * mc::kMaxG ? mc::ring_stages(mc::kRingRows * cols * (x_dtype == MC_BF16 ? 2 : 4)) : 0;
-  if (ring > 0) {
-    const int smem = ring * mc::kRingRows * cols * (x_dtype == MC_BF16 ? 2 : 4) + ring * 16 + 64;
-    const int64_t chunks = (rows + mc::kRingRows - 1) / mc::kRingRows;
-    const int grid = static_cast<int>(chunks < mc::num_sms() ? chunks : mc::num_sms());
-    int32_t rc = MC_OK;
-#define MC_LNT(G, IDX)                                                                                                                 \
-  do {                                                                                                                                 \
-    static mc::PerDeviceOnce once_##IDX;                                                                                               \
-    rc = mc::set_max_smem_once(mc::ln_modulate_tma_kernel<G, mc::kLnRingGroups>, 208 * 1024, once_##IDX, "cudaFuncSetAttribute(ln_modulate_tma smem)");   \
-    if (rc == MC_OK)                                                                                                                   \
-      mc::ln_modulate_tma_kernel<G, mc::kLnRingGroups><<<grid, mc::ring_threads(mc::kLnRingGroups), smem, s>>>(x, x_dtype == MC_BF16, rows, cols, eps, mode, p0, p1, scale_idx, \
-                                                                        shift_idx, round_ln_to_bf16, out, out_dtype == MC_BF16, ring); \
-  } while (0)
-    if (groups <= 32 * 2) MC_LNT(2, 2);
-    else if (groups <= 32 * 4) MC_LNT(4, 4);
-    else if (groups <= 32 * 6) MC_LNT(6, 6);
-    else MC_LNT(8, 8);
-#undef MC_LNT
-    if (rc) return rc;
-    MC_CHECK_LAUNCH("ln_modulate_tma_kernel launch");
-    return MC_OK;
+  const int stage_bytes = mc::kRingRows * cols * (x_bf16 ? 2 : 4);
+  const int ring = rows >= 1024 && groups <= 32 * mc::kMaxG ? mc::ring_stages(stage_bytes, mc::kRowRingMaxStages) : 0;
+  if (ring > 0)
+    return mc::with_lane_groups(groups, [&](auto G) {
+      return mc::launch_ring<mc::ln_modulate_tma_kernel<decltype(G)::value, mc::kLnRingGroups>>(
+          ring, stage_bytes, 0, (rows + mc::kRingRows - 1) / mc::kRingRows, mc::ring_threads(mc::kLnRingGroups), s, "ln_modulate_tma_kernel",
+          x, x_bf16, rows, cols, eps, mode, p0, p1, scale_idx, shift_idx, round_ln_to_bf16, out, o_bf16, ring);
+    });
+  if (groups <= 32 * mc::kMaxG) {
+    mc::with_lane_groups(groups, [&](auto G) {
+      constexpr int g = decltype(G)::value;
+      mc::ln_modulate_pipe_kernel<g><<<mc::pipe_grid(rows, g >= 6 ? 1 : 2), 256, 0, s>>>(x, x_bf16, rows, cols, eps, mode, p0, p1, scale_idx,
+                                                                                       shift_idx, round_ln_to_bf16, out, o_bf16);
+    });
+  } else {
+    mc::ln_modulate_kernel<<<mc::grid_for(rows, 256 / (32 * mc::kWideWarps)), 256, 0, s>>>(x, x_bf16, rows, cols, eps, mode, p0, p1, scale_idx,
+                                                                                          shift_idx, round_ln_to_bf16, out, o_bf16);
   }
-  if (groups <= 32 * 2) MC_LNP(2);
-  else if (groups <= 32 * 4) MC_LNP(4);
-  else if (groups <= 32 * 6) MC_LNP(6);
-  else if (groups <= 32 * mc::kMaxG) MC_LNP(8);
-  else MC_LN(128);
-#undef MC_LNP
-#undef MC_LN
   MC_CHECK_LAUNCH("ln_modulate_kernel launch");
   return MC_OK;
 }
@@ -883,7 +747,7 @@ int32_t mc_rmsnorm_rope_segs(void* x_bf16, int64_t ld, int64_t rows, int32_t seg
                              int32_t head_dim, void* stream) {
   MC_CHECK_ARG(x_bf16 && w, "mc_rmsnorm_rope: null pointer");
   MC_CHECK_ARG(segs >= 1 && segs <= 4, "mc_rmsnorm_rope: segs=%d outside [1, 4]", segs);
-  MC_CHECK_ARG(rows >= 1 && cols >= 8 && cols % 8 == 0 && cols <= 128 * 8 * mc::kMaxG && ld >= static_cast<int64_t>(segs) * cols && ld % 8 == 0,
+  MC_CHECK_ARG(rows >= 1 && cols >= 8 && cols % 8 == 0 && cols <= 32 * mc::kWideWarps * 8 * mc::kMaxG && ld >= static_cast<int64_t>(segs) * cols && ld % 8 == 0,
                "mc_rmsnorm_rope: cols=%d ld=%lld unsupported", cols, static_cast<long long>(ld));
   MC_CHECK_ARG(mc::aligned16(x_bf16), "mc_rmsnorm_rope: x must be 16-byte aligned");
   MC_CHECK_ARG(mc::aligned16(w), "mc_rmsnorm_rope: weight must be 16-byte aligned");
@@ -896,40 +760,23 @@ int32_t mc_rmsnorm_rope_segs(void* x_bf16, int64_t ld, int64_t rows, int32_t seg
                        (cos_sin == nullptr || 256 % head_dim == 0);
   const int rows_per_stage = mc::kRingRows / (segs == 3 ? 1 : segs);
   const int ring_stage_bytes = mc::kRingRows * cols * 2 + (cos_sin != nullptr ? rows_per_stage * head_dim * 4 : 0);
-  const int ring = ring_ok ? mc::ring_stages(ring_stage_bytes) : 0;
-  if (ring > 0) {
-    const int smem = ring * ring_stage_bytes + ring * 16 + 64;
-    const int64_t chunks = (rows + rows_per_stage - 1) / rows_per_stage;
-    const int grid = static_cast<int>(chunks < mc::num_sms() ? chunks : mc::num_sms());
-    int32_t rc = MC_OK;
-#define MC_RMST(G, IDX)                                                                                                                 \
-  do {                                                                                                                                  \
-    static mc::PerDeviceOnce once_##IDX;                                                                                                \
-    rc = mc::set_max_smem_once(mc::rmsnorm_rope_tma_kernel<G, mc::kRmsRingGroups>, 208 * 1024, once_##IDX, "cudaFuncSetAttribute(rmsnorm_rope_tma smem)"); \
-    if (rc == MC_OK)                                                                                                                    \
-      mc::rmsnorm_rope_tma_kernel<G, mc::kRmsRingGroups><<<grid, mc::ring_threads(mc::kRmsRingGroups), smem, s>>>(xp, ld, rows, segs, cols, w, eps, cos_sin, head_dim, ring);   \
-  } while (0)
-    if (groups <= 32 * 2) MC_RMST(2, 2);
-    else if (groups <= 32 * 4) MC_RMST(4, 4);
-    else if (groups <= 32 * 6) MC_RMST(6, 6);
-    else MC_RMST(8, 8);
-#undef MC_RMST
-    if (rc) return rc;
-    MC_CHECK_LAUNCH("rmsnorm_rope_tma_kernel launch");
-    return MC_OK;
-  }
-#define MC_RMSP(G) mc::rmsnorm_rope_pipe_kernel<G><<<mc::pipe_grid(rows * segs), 256, 0, s>>>(xp, ld, rows, segs, cols, w, eps, cos_sin, head_dim)
-  if (groups <= 32 * 2) MC_RMSP(2);
-  else if (groups <= 32 * 4) MC_RMSP(4);
-  else if (groups <= 32 * 6) MC_RMSP(6);
-  else if (groups <= 32 * mc::kMaxG) MC_RMSP(8);
-  else {
+  const int ring = ring_ok ? mc::ring_stages(ring_stage_bytes, mc::kRowRingMaxStages) : 0;
+  if (ring > 0)
+    return mc::with_lane_groups(groups, [&](auto G) {
+      return mc::launch_ring<mc::rmsnorm_rope_tma_kernel<decltype(G)::value, mc::kRmsRingGroups>>(
+          ring, ring_stage_bytes, 0, (rows + rows_per_stage - 1) / rows_per_stage, mc::ring_threads(mc::kRmsRingGroups), s,
+          "rmsnorm_rope_tma_kernel", xp, ld, rows, segs, cols, w, eps, cos_sin, head_dim, ring);
+    });
+  if (groups <= 32 * mc::kMaxG) {
+    mc::with_lane_groups(groups, [&](auto G) {
+      mc::rmsnorm_rope_pipe_kernel<decltype(G)::value><<<mc::pipe_grid(rows * segs), 256, 0, s>>>(xp, ld, rows, segs, cols, w, eps, cos_sin, head_dim);
+    });
+  } else {
     // wide rows (Wan-14B: 5120): four warps per row, one column block per launch
     for (int sg = 0; sg < segs; ++sg)
-      mc::rmsnorm_rope_kernel<128><<<mc::grid_for(rows, 2), 256, 0, s>>>(xp + static_cast<int64_t>(sg) * cols, ld, rows, cols,
-                                                                        w + static_cast<int64_t>(sg) * cols, eps, cos_sin, head_dim);
+      mc::rmsnorm_rope_kernel<<<mc::grid_for(rows, 256 / (32 * mc::kWideWarps)), 256, 0, s>>>(
+          xp + static_cast<int64_t>(sg) * cols, ld, rows, cols, w + static_cast<int64_t>(sg) * cols, eps, cos_sin, head_dim);
   }
-#undef MC_RMSP
   MC_CHECK_LAUNCH("rmsnorm_rope_kernel launch");
   return MC_OK;
 }

@@ -193,12 +193,15 @@ def _ref_stats(r, p, eps=0.0):
     return ratio.mean().item(), ratio.std().item(), (1 - torch.nn.functional.cosine_similarity(r, p, dim=-1, eps=1e-8)).mean().item()
 
 
-@pytest.mark.parametrize("shape", [(1, 64, 96), (2, 33, 1536), (1, 32760, 1536)])
-def test_residual_stats(shape):
+# fp32 up to ~3000 columns: the staged kernel; 5120 fp32 columns (fewer than two stages fit) and bf16: the warp-per-row kernel
+@pytest.mark.parametrize("shape,dtype", [((1, 64, 96), torch.float32), ((2, 33, 1536), torch.float32), ((1, 32760, 1536), torch.float32),
+                                         ((1, 777, 5120), torch.float32), ((2, 515, 1536), torch.bfloat16)])
+def test_residual_stats(shape, dtype):
     ops = _ops()
     g = torch.Generator(device=DEV).manual_seed(5)
     p = torch.randn(*shape, device=DEV, generator=g) * 0.1
     r = p * (0.97 + 0.05 * torch.rand(shape[0], shape[1], 1, device=DEV, generator=g)) + 0.01 * torch.randn(*shape, device=DEV, generator=g)
+    r, p = r.to(dtype), p.to(dtype)
     got = ops.residual_stats(r, p)
     ref = _ref_stats(r.double(), p.double())
     for a, b in zip(got, ref):
@@ -553,7 +556,8 @@ def test_rmsnorm_rope_two_blocks_one_launch(rows, D):
 
 def test_rmsnorm_rope_staged_form_matches_register_form_bitwise():
     """The TMA-staged kernels (>= 1024 items) and the register-pipelined ones (fewer) run the same per-row arithmetic: the first
-    1000 rows of a long input, processed alone, must come out bit-identical; likewise LayerNorm + modulation."""
+    1000 rows of a long input, processed alone, must come out bit-identical; likewise LayerNorm + modulation (mode 0) and the
+    affine LayerNorm (mode 1), from fp32 and from bf16 input with the LN value rounded to bf16, into bf16 and into fp32."""
     ops = _ops()
     g = torch.Generator(device=DEV).manual_seed(3)
     D = 1536
@@ -569,6 +573,15 @@ def test_rmsnorm_rope_staged_form_matches_register_form_bitwise():
     ya = ops.ln_modulate(x, em, 4, 3)
     yb = ops.ln_modulate(x[:1000], em, 4, 3)
     assert torch.equal(ya[:1000], yb)
+    xh = x.bfloat16()
+    for out_dtype in (torch.bfloat16, torch.float32):
+        ya = ops.ln_modulate(xh, em, 1, 0, round_ln_to_bf16=True, out_dtype=out_dtype)
+        yb = ops.ln_modulate(xh[:1000], em, 1, 0, round_ln_to_bf16=True, out_dtype=out_dtype)
+        assert ya.dtype == out_dtype and torch.equal(ya[:1000], yb)
+        for xi in (x, xh):
+            ya = ops.ln_affine(xi, em[0], em[5], out_dtype=out_dtype)
+            yb = ops.ln_affine(xi[:1000], em[0], em[5], out_dtype=out_dtype)
+            assert torch.equal(ya[:1000], yb)
 
 
 # ------------------------------------------------------------------------------------------- wgmma attention
