@@ -199,6 +199,13 @@ int32_t mc_tea_decide(const mc_tea_config* cfg, mc_tea_state* st, double rel_l1,
 int32_t mc_tea_advance(const mc_tea_config* cfg, mc_tea_state* st);
 /* sums_dev (device, 2 doubles, overwritten) = { sum |cur - prev|, sum |prev| } over n fp32 elements — the two means of :543. */
 int32_t mc_rel_l1(const float* cur, const float* prev, int64_t n, double* sums_dev, void* stream);
+/* Open-Sora's TeaCache rule (eval/magcache/experiments/opensora.py:96-107), one call:
+ *   forced (timestep[0] == all_timesteps[0] or == all_timesteps[-1]) -> *calc = 1, *accumulated_out = 0
+ *   else accumulated += np.poly1d(coef)(rel); *calc = !(accumulated < thresh); on a compute the sum is reset to 0
+ * rel is the value `.cpu().item()` returns (the bf16 quotient of the two bf16 means), ignored when forced. coef: n_coef (1..8)
+ * coefficients, highest power first. float64 throughout, bit-exact with the reference. */
+int32_t mc_tea_opensora_decide(int32_t forced, double rel, double accumulated, double thresh, const double* coef, int32_t n_coef,
+                               int32_t* calc, double* accumulated_out);
 
 /* ------------------------------------------------------------------------------------------------------------
  * DiT block-stack kernels (cache-miss branch `for block in self.blocks: x = block(x, **kwargs)`,
@@ -222,6 +229,20 @@ int32_t mc_patchify(const float* latent, int32_t C, int32_t F, int32_t H, int32_
 int32_t mc_ln_modulate(const void* x, int32_t x_dtype, int64_t rows, int32_t cols, float eps, int32_t mode,
                        const float* p0, const float* p1, int32_t scale_idx, int32_t shift_idx,
                        int32_t round_ln_to_bf16, void* out, int32_t out_dtype, void* stream);
+
+/* Mode 2 of mc_ln_modulate (same per-row arithmetic, same output bits) fused with the input distance of Open-Sora's TeaCache
+ * (eval/magcache/experiments/opensora.py:95, :102):
+ *   out = t2i_modulate(spatial_blocks[0].norm1(x), shift, scale)                    `modulated_inp`
+ *   sums_dev[0] += sum float(|bf16(out - prev)|),  sums_dev[1] += sum float(|prev|)  `(modulated_inp - previous_modulated_input).abs()`,
+ *                                                                                    `previous_modulated_input.abs()` before `.mean()`
+ * prev: the previous call's bf16 output, [rows, cols]; out may not alias x or prev. The sums are added, so per-sample launches into one
+ * zeroed sums_dev give the sums over all samples. Deterministic: per-CTA partials (fp64) in partials_dev, at least
+ * 2 * MC_LN_REL_L1_MAX_CTAS doubles of device scratch, then one fixed-order sum; the same inputs give the same bits on every launch.
+ * x, out, prev, p0, partials_dev 16-byte aligned; cols % 8 == 0, cols <= 2048. */
+#define MC_LN_REL_L1_MAX_CTAS 4096
+int32_t mc_ln_t2i_modulate_rel_l1(const void* x, int64_t rows, int32_t cols, float eps, const float* p0, int32_t scale_idx,
+                                  int32_t shift_idx, const void* prev, void* out, double* partials_dev, double* sums_dev,
+                                  void* stream);
 
 /* WanRMSNorm over the full model dim followed by 3-axis RoPE (rope_apply), in place on bf16 [rows, cols]:
  *   y = bf16(rope(float(bf16(x * rsqrt(mean(x^2)+eps))) * w)).  cos_sin == NULL -> no RoPE (cross-attention q/k).

@@ -84,6 +84,9 @@ SIGNATURES = {
     "mc_tea_decide": [POINTER(TeaConfig), POINTER(TeaState), c_double, POINTER(c_int32)],
     "mc_tea_advance": [POINTER(TeaConfig), POINTER(TeaState)],
     "mc_rel_l1": [c_void_p, c_void_p, c_int64, c_void_p, c_void_p],
+    "mc_tea_opensora_decide": [c_int32, c_double, c_double, c_double, POINTER(c_double), c_int32, POINTER(c_int32), POINTER(c_double)],
+    "mc_ln_t2i_modulate_rel_l1": [c_void_p, c_int64, c_int32, c_float, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                  c_void_p],
     "mc_cache_hit_add": [c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_int64, c_void_p],
     "mc_residual_sub": [c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_int64, c_void_p],
     "mc_cfg_combine": [c_void_p, c_void_p, c_float, c_void_p, c_int64, c_void_p],

@@ -190,6 +190,41 @@ class AttrController:
             self._store(o, st, with_cnt=True)
 
 
+def _bf16(v):
+    """fp32 -> bf16 (round to nearest even), as a Python float."""
+    b = np.array([v], dtype=np.float32).view(np.uint32)
+    b = (b + np.uint32(0x7FFF) + ((b >> np.uint32(16)) & np.uint32(1))) & np.uint32(0xFFFF0000)
+    return float(b.view(np.float32)[0])
+
+
+def opensora_rel_l1(sum_d, sum_p, n):
+    """`((cur - prev).abs().mean() / prev.abs().mean()).cpu().item()` on bf16 tensors (eval/magcache/experiments/opensora.py:102) from
+    the two sums over n elements: each mean is an fp32 quotient rounded to a bf16 scalar, and so is their quotient."""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        m_d = _bf16(np.float32(sum_d) / np.float32(n))
+        m_p = _bf16(np.float32(sum_p) / np.float32(n))
+        return _bf16(np.float32(m_d) / np.float32(m_p))
+
+
+class OpenSoraTeaController:
+    """Open-Sora's TeaCache rule (eval/magcache/experiments/opensora.py:96-107) through `mc_tea_opensora_decide`, on state under the
+    reference's attribute names: `rel_l1_thresh`, `accumulated_rel_l1_distance`. No counter: a call is forced by its timestep."""
+
+    COEFFICIENTS = (2.17546007e+02, -1.18329252e+02, 2.68662585e+01, -4.59364272e-02, 4.84426240e-02)  # :100
+
+    def __init__(self, coefficients=COEFFICIENTS):
+        self._coef = (ctypes.c_double * len(coefficients))(*[float(c) for c in coefficients])
+        self._n = len(coefficients)
+
+    def decide(self, o, forced, rel):
+        """True = compute the blocks. `rel` (the bf16 distance, `opensora_rel_l1`) is ignored on a forced call."""
+        calc, acc = ctypes.c_int32(), ctypes.c_double()
+        check(lib.mc_tea_opensora_decide(int(bool(forced)), 0.0 if rel is None else float(rel), float(o.accumulated_rel_l1_distance),
+                                         float(o.rel_l1_thresh), self._coef, self._n, ctypes.byref(calc), ctypes.byref(acc)))
+        o.accumulated_rel_l1_distance = acc.value
+        return bool(calc.value)
+
+
 class TeaController:
     """TeaCache's rule (eval/magcache/experiments/Wan2.1_EVAL/wan_teacache.py:535-564, 587-589) on state under that script's attribute
     names: `cnt, num_steps, ret_steps, cutoff_steps, coefficients, teacache_thresh, accumulated_rel_l1_distance_even / _odd`."""

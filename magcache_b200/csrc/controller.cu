@@ -323,6 +323,29 @@ int32_t mc_tea_decide(const mc_tea_config* cfg, mc_tea_state* st, double rel_l1,
   return MC_OK;
 }
 
+// ---- Open-Sora's rule: eval/magcache/experiments/opensora.py:96-107 (forced on the first / last sampler timestep, no counter) ---
+int32_t mc_tea_opensora_decide(int32_t forced, double rel, double accumulated, double thresh, const double* coef, int32_t n_coef,
+                               int32_t* calc, double* accumulated_out) {
+  MC_CHECK_ARG(calc && accumulated_out, "mc_tea_opensora_decide: null pointer");
+  if (forced) {
+    *calc = 1;
+    *accumulated_out = 0.0;
+    return MC_OK;
+  }
+  MC_CHECK_ARG(coef && n_coef >= 1 && n_coef <= 8, "mc_tea_opensora_decide: n_coef=%d outside [1, 8]", n_coef);
+  double y = 0.0;  // np.poly1d(coefficients)(rel): Horner, highest power first
+  for (int k = 0; k < n_coef; ++k) y = y * rel + coef[k];
+  accumulated += y;
+  if (accumulated < thresh) {
+    *calc = 0;
+  } else {
+    *calc = 1;
+    accumulated = 0.0;
+  }
+  *accumulated_out = accumulated;
+  return MC_OK;
+}
+
 int32_t mc_tea_advance(const mc_tea_config* cfg, mc_tea_state* st) {
   MC_CHECK_ARG(cfg && st, "mc_tea_advance: null pointer");
   st->cnt += 1;

@@ -139,24 +139,38 @@ __global__ void __launch_bounds__(256) ln_modulate_kernel(const void* __restrict
 // ---- mode 2: LayerNorm + t2i_modulate with every step a bf16 tensor op (STDiT3Block.forward, open_sora_transformer_3d.py:187, :248;
 // T2IFinalLayer, :80): y = bf16(bf16(bf16(LN(x)) * bf16(1 + p0[scale_idx])) + p0[shift_idx]), p0 holding bf16 values.
 // One warp per row, x and out bf16, cols <= 2048.
-__global__ void __launch_bounds__(256) ln_t2i_modulate_kernel(const __nv_bfloat16* __restrict__ x, int64_t rows, int cols, float eps,
+// kRelL1: TeaCache's input distance (eval/magcache/experiments/opensora.py:102) against `prev`, the previous call's output of the
+// same shape, taken while the output row is in registers: each warp adds Σ float(|bf16(out - prev)|) and Σ float(|prev|) of its rows
+// (fp32 within a row, fp64 across rows), the CTA's warps are added in warp order into partials[blockIdx.x] = {Σ|d|, Σ|prev|}, and
+// rel_l1_finish_kernel adds the partials in a fixed order: no floating-point atomics, the same bits on every launch.
+// G: 8-element groups per lane (cols <= 256 G); the plain form is instantiated at kMaxG. The distance forms up to G = 6 fit two
+// CTAs per SM (<= 128 registers), like the plain form.
+template <int G, bool kRelL1>
+__global__ void __launch_bounds__(256, (kRelL1 && G < 8) ? 2 : 0) ln_t2i_modulate_kernel(const __nv_bfloat16* __restrict__ x, int64_t rows, int cols, float eps,
                                                               const float* __restrict__ sc, const float* __restrict__ sh,
-                                                              __nv_bfloat16* __restrict__ out) {
+                                                              __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ prev,
+                                                              double2* __restrict__ partials) {
   const int lane = threadIdx.x & 31;
   const int groups = cols >> 3;
   const float inv_n = 1.0f / static_cast<float>(cols);
+  double acc_d = 0.0, acc_p = 0.0;  // kRelL1: this warp's rows (lane 0)
   for (int64_t row = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; row < rows;
        row += (static_cast<int64_t>(gridDim.x) * blockDim.x) >> 5) {
-    float v[kMaxG][8];
+    float v[G][8];
+    uint4 pv[kRelL1 ? G : 1];
 #pragma unroll
-    for (int i = 0; i < kMaxG; ++i) {
+    for (int i = 0; i < G; ++i) {
       const int g = lane + i * 32;
-      if (g < groups) unpack_bf16x8(ptx::ld_nc_v4(x + row * cols + g * 8), v[i]);
+      if (g < groups) {
+        unpack_bf16x8(ptx::ld_nc_v4(x + row * cols + g * 8), v[i]);
+        if constexpr (kRelL1) pv[i] = ptx::ld_nc_v4(prev + row * cols + g * 8);
+      }
     }
     float mean;
-    const float rstd = ln_rstd<kMaxG>(v, lane, 32, groups, inv_n, eps, WarpReduce(), mean);
+    const float rstd = ln_rstd<G>(v, lane, 32, groups, inv_n, eps, WarpReduce(), mean);
+    float sd = 0.f, sp = 0.f;
 #pragma unroll
-    for (int i = 0; i < kMaxG; ++i) {
+    for (int i = 0; i < G; ++i) {
       const int g = lane + i * 32;
       if (g < groups) {
         float a[8], b[8], o[8];
@@ -168,8 +182,60 @@ __global__ void __launch_bounds__(256) ln_t2i_modulate_kernel(const __nv_bfloat1
           o[j] = round_bf16(__fadd_rn(round_bf16(__fmul_rn(y, round_bf16(__fadd_rn(1.0f, a[j])))), b[j]));
         }
         ptx::st_na_v4(out + row * cols + g * 8, pack_bf16x8(o));
+        if constexpr (kRelL1) {
+          float p[8];
+          unpack_bf16x8(pv[i], p);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            sd += fabsf(round_bf16(__fsub_rn(o[j], p[j])));  // `(cur - prev)` is a bf16 tensor op, then `.abs()`
+            sp += fabsf(p[j]);
+          }
+        }
       }
     }
+    if constexpr (kRelL1) {
+      sd = warp_sum(sd);
+      sp = warp_sum(sp);
+      acc_d += static_cast<double>(sd);
+      acc_p += static_cast<double>(sp);
+    }
+  }
+  if constexpr (kRelL1) {
+    __shared__ double2 warp_acc[8];
+    if (lane == 0) warp_acc[threadIdx.x >> 5] = make_double2(acc_d, acc_p);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double2 t = warp_acc[0];
+      for (int w = 1; w < static_cast<int>(blockDim.x >> 5); ++w) {
+        t.x += warp_acc[w].x;
+        t.y += warp_acc[w].y;
+      }
+      partials[blockIdx.x] = t;
+    }
+  }
+}
+
+// sums[0..1] += the n partials of ln_t2i_modulate_kernel<true>, added in a fixed order: 256 threads each take a fixed strided
+// subset, then a shared-memory tree. One CTA.
+__global__ void __launch_bounds__(256) rel_l1_finish_kernel(const double2* __restrict__ partials, int n, double* __restrict__ sums) {
+  __shared__ double2 s[256];
+  double2 t = make_double2(0.0, 0.0);
+  for (int i = threadIdx.x; i < n; i += 256) {
+    t.x += partials[i].x;
+    t.y += partials[i].y;
+  }
+  s[threadIdx.x] = t;
+  __syncthreads();
+  for (int h = 128; h > 0; h >>= 1) {
+    if (static_cast<int>(threadIdx.x) < h) {
+      s[threadIdx.x].x += s[threadIdx.x + h].x;
+      s[threadIdx.x].y += s[threadIdx.x + h].y;
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    sums[0] += s[0].x;
+    sums[1] += s[0].y;
   }
 }
 
@@ -698,9 +764,9 @@ int32_t mc_ln_modulate(const void* x, int32_t x_dtype, int64_t rows, int32_t col
                  "mc_ln_modulate: mode 2 needs bf16 x / out and cols %% 8 == 0, cols <= 2048 (cols=%d)", cols);
     MC_CHECK_ARG(mc::aligned16(x) && mc::aligned16(out) && mc::aligned16(p0) && cols % 4 == 0, "mc_ln_modulate: mode 2 pointers must be 16-byte aligned");
     const int64_t want = (rows + 7) / 8, cap = static_cast<int64_t>(mc::num_sms()) * 16;
-    mc::ln_t2i_modulate_kernel<<<static_cast<int>(want < cap ? want : cap), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+    mc::ln_t2i_modulate_kernel<mc::kMaxG, false><<<static_cast<int>(want < cap ? want : cap), 256, 0, static_cast<cudaStream_t>(stream)>>>(
         static_cast<const __nv_bfloat16*>(x), rows, cols, eps, p0 + static_cast<int64_t>(scale_idx) * cols,
-        p0 + static_cast<int64_t>(shift_idx) * cols, static_cast<__nv_bfloat16*>(out));
+        p0 + static_cast<int64_t>(shift_idx) * cols, static_cast<__nv_bfloat16*>(out), nullptr, nullptr);
     MC_CHECK_LAUNCH("ln_t2i_modulate_kernel launch");
     return MC_OK;
   }
@@ -732,6 +798,31 @@ int32_t mc_ln_modulate(const void* x, int32_t x_dtype, int64_t rows, int32_t col
                                                                                           shift_idx, round_ln_to_bf16, out, o_bf16);
   }
   MC_CHECK_LAUNCH("ln_modulate_kernel launch");
+  return MC_OK;
+}
+
+int32_t mc_ln_t2i_modulate_rel_l1(const void* x, int64_t rows, int32_t cols, float eps, const float* p0, int32_t scale_idx, int32_t shift_idx,
+                                  const void* prev, void* out, double* partials_dev, double* sums_dev, void* stream) {
+  MC_CHECK_ARG(x && p0 && prev && out && partials_dev && sums_dev, "mc_ln_t2i_modulate_rel_l1: null pointer");
+  MC_CHECK_ARG(rows >= 1 && cols >= 8 && cols % 8 == 0 && cols <= 32 * 8 * mc::kMaxG, "mc_ln_t2i_modulate_rel_l1: cols %% 8 == 0, cols <= 2048 (cols=%d)",
+               cols);
+  MC_CHECK_ARG(mc::aligned16(x) && mc::aligned16(out) && mc::aligned16(prev) && mc::aligned16(p0) && mc::aligned16(partials_dev),
+               "mc_ln_t2i_modulate_rel_l1: pointers must be 16-byte aligned");
+  MC_CHECK_ARG(prev != out && x != out, "mc_ln_t2i_modulate_rel_l1: out may not alias x or prev");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int64_t grid = (rows + 7) / 8;
+  const int64_t cap = static_cast<int64_t>(mc::num_sms()) * 16;
+  if (grid > cap) grid = cap;
+  if (grid > MC_LN_REL_L1_MAX_CTAS) grid = MC_LN_REL_L1_MAX_CTAS;
+  double2* parts = reinterpret_cast<double2*>(partials_dev);
+  mc::with_lane_groups(cols / 8, [&](auto G) {
+    mc::ln_t2i_modulate_kernel<decltype(G)::value, true><<<static_cast<int>(grid), 256, 0, s>>>(
+        static_cast<const __nv_bfloat16*>(x), rows, cols, eps, p0 + static_cast<int64_t>(scale_idx) * cols,
+        p0 + static_cast<int64_t>(shift_idx) * cols, static_cast<__nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(prev), parts);
+  });
+  MC_CHECK_LAUNCH("ln_t2i_modulate_kernel<rel_l1> launch");
+  mc::rel_l1_finish_kernel<<<1, 256, 0, s>>>(parts, static_cast<int>(grid), sums_dev);
+  MC_CHECK_LAUNCH("rel_l1_finish_kernel launch");
   return MC_OK;
 }
 

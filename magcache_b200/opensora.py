@@ -228,17 +228,24 @@ class OpenSoraEngine:
         self.fin_t.view(B, 2, D).copy_(t.view(B, 1, D).expand(B, 2, D))
         ops.cast_into(ops.cache_hit_add(self.fin_rep, self.fin_t, out=self.fin), self.finf)  # final layer `table[None] + t[:, None]`
         if kind == "miss":
-            f1w, f1b, f2w, f2b = w.y_mlp
-            self.y_emb = ops.gemm(ops.gemm(self.y_in, f1w, f1b, E.MC_EPI_BIAS_GELU_BF16), f2w, f2b, E.MC_EPI_BIAS_BF16)
+            self.caption()
+
+    def caption(self):
+        """The caption MLP (`y_embedder`), which only the block stack reads."""
+        f1w, f1b, f2w, f2b = self.w.y_mlp
+        self.y_emb = ops.gemm(ops.gemm(self.y_in, f1w, f1b, E.MC_EPI_BIAS_GELU_BF16), f2w, f2b, E.MC_EPI_BIAS_BF16)
 
     # ------------------------------------------------------------------------------------------ blocks (STDiT3Block.forward)
-    def _block(self, i, blk):
+    def _block(self, i, blk, x_m=None):
+        """`x_m`: this block's first LN + t2i_modulate output when the caller already has it (TeaCache's decision input is block 0's)."""
         w, B, D, H = self.w, self.B, self.w.dim, self.w.heads
         x, h, qkv, att = self.x, self.h, self.qkv, self.att
         em = [self.modf[i, b].view(6, D) for b in range(B)]  # shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp
-        for b in range(B):
-            ops.ln_t2i_modulate(x[self.rows(b)], em[b], 1, 0, out=h[self.rows(b)])
-        ops.gemm(h, blk["qkv_w"], blk["qkv_b"], E.MC_EPI_BIAS_BF16, out=qkv)
+        if x_m is None:
+            for b in range(B):
+                ops.ln_t2i_modulate(x[self.rows(b)], em[b], 1, 0, out=h[self.rows(b)])
+            x_m = h
+        ops.gemm(x_m, blk["qkv_w"], blk["qkv_b"], E.MC_EPI_BIAS_BF16, out=qkv)
         q, k, v = qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:]
         rope = self.rope if blk["temporal"] else None
         ops.rmsnorm_head72_rope_(q, blk["nq"], H, rope, pos_div=self.S, tag="os_qknorm")
@@ -261,10 +268,10 @@ class OpenSoraEngine:
         for b in range(B):
             ops.gemm(self.ff[self.rows(b)], blk["f2_w"], blk["f2_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=x[self.rows(b)], gate=em[b][5])
 
-    def run_blocks(self):
+    def run_blocks(self, x_m0=None):
         self.x.copy_(self.x0)
         for i, blk in enumerate(self.w.blocks):
-            self._block(i, blk)
+            self._block(i, blk, x_m0 if i == 0 else None)
         return self.x
 
     # ------------------------------------------------------------------------------------------ output (T2IFinalLayer, unpatchify)
@@ -290,6 +297,64 @@ class OpenSoraEngine:
             ops.residual_sub(x, self.x0, out=self.res)
             self.res_valid = True
         return self.head(x)
+
+    # ------------------------------------------------------------------------------------------ TeaCache (opensora.py:34-227)
+    def _tea_alloc(self):
+        if self.__dict__.get("_tea_shape") == self._shape:
+            return
+        self.mi = torch.empty(2, self.R, self.w.dim, dtype=torch.bfloat16, device=self.device)  # modulated inputs, alternating
+        self.mi_prev = None  # index of the buffer holding `previous_modulated_input`, None: there is none
+        self.tea_sums = torch.zeros(2, dtype=torch.float64, device=self.device)
+        self.tea_partials = ops.rel_l1_partials(self.device)
+        self._tea_shape = self._shape
+
+    def take_modulated_input(self, cur):
+        """Follow the `previous_modulated_input` attribute: None clears it; a tensor other than the engine's own buffer is copied in."""
+        self._tea_alloc()
+        if cur is None:
+            self.mi_prev = None
+        elif self.mi_prev is None or cur.data_ptr() != self.mi[self.mi_prev].data_ptr():
+            self.mi_prev = 0 if self.mi_prev is None else self.mi_prev
+            self.mi[self.mi_prev].copy_(cur.reshape(self.R, self.w.dim))
+
+    def modulated_input(self, distance):
+        """TeaCache's decision input `t2i_modulate(spatial_blocks[0].norm1(x0), shift_msa, scale_msa)` (:89-95) per sample, into the
+        buffer that does not hold the previous one, which it then replaces (:108). With `distance`, the same launches also return the
+        two sums (sum |cur - prev|, sum |prev|) over all samples (:102), one host sync. Call after `prologue`."""
+        self._tea_alloc()
+        k = 0 if self.mi_prev is None else 1 - self.mi_prev
+        cur, D = self.mi[k], self.w.dim
+        if distance:
+            prev = self.mi[self.mi_prev]
+            self.tea_sums.zero_()
+            for b in range(self.B):
+                ops.ln_t2i_modulate_rel_l1(self.x0[self.rows(b)], self.modf[0, b].view(6, D), 1, 0, prev[self.rows(b)], cur[self.rows(b)],
+                                           self.tea_partials, self.tea_sums, tag="os_tea_input")
+        else:
+            for b in range(self.B):
+                ops.ln_t2i_modulate(self.x0[self.rows(b)], self.modf[0, b].view(6, D), 1, 0, out=cur[self.rows(b)], tag="os_tea_input")
+        self.mi_prev = k
+        return self.tea_sums.tolist() if distance else None
+
+    def forward_teacache(self, calc):
+        """After `prologue("hit")` and `modulated_input`: hit `x += previous_residual` (bf16, :114) | miss: the caption MLP, the block
+        stack with block 0's first LN-modulate taken from the decision input (the same tensor), `previous_residual = x - origin_x`
+        (:156) -> final layer."""
+        if not calc:
+            if not self.res_valid:
+                raise TypeError("magcache_b200: TeaCache hit with no previous_residual")
+            x = ops.cache_hit_add(self.x0, self.res, out=self.hit)
+        else:
+            self.caption()
+            x = self.run_blocks(self.mi[self.mi_prev])
+            ops.residual_sub(x, self.x0, out=self.res)
+            self.res_valid = True
+        return self.head(x)
+
+    def forward_plain(self):
+        """`enable_teacache = False` (:157-197): the block stack, no residual kept."""
+        self.prologue("miss")
+        return self.head(self.run_blocks())
 
 
 def random_opensora_weights(dev, hidden_size=1152, depth=28, num_heads=16, caption_channels=4096, model_max_length=300, seed=0):

@@ -333,6 +333,29 @@ def ln_t2i_modulate(x, em, scale_idx, shift_idx, eps=1e-6, out=None, tag=None):
     return out
 
 
+REL_L1_MAX_CTAS = 4096  # MC_LN_REL_L1_MAX_CTAS
+
+
+def rel_l1_partials(device):
+    """Device scratch for `ln_t2i_modulate_rel_l1`'s per-CTA partial sums."""
+    return torch.empty(2 * REL_L1_MAX_CTAS, dtype=torch.float64, device=device)
+
+
+def ln_t2i_modulate_rel_l1(x, em, scale_idx, shift_idx, prev, out, partials, sums, eps=1e-6, tag=None):
+    """`ln_t2i_modulate` into `out` fused with TeaCache's input distance against `prev` (`mc_ln_t2i_modulate_rel_l1`):
+    sums (fp64 [2], on the device) += (sum |bf16(out - prev)|, sum |prev|). Deterministic; no host sync."""
+    _dev(x), _dev(prev), _dev(out)
+    rows, cols = x.shape
+    assert x.dtype == prev.dtype == out.dtype == torch.bfloat16 and x.is_contiguous() and prev.is_contiguous() and out.is_contiguous()
+    assert prev.shape == out.shape == x.shape and em.dtype == torch.float32 and em.is_contiguous() and em.shape[-1] == cols
+    assert sums.dtype == partials.dtype == torch.float64 and sums.numel() >= 2 and partials.numel() >= 2 * REL_L1_MAX_CTAS
+    with _Timed(tag, "ln_t2i_modulate_rel_l1"):
+        check(lib.mc_ln_t2i_modulate_rel_l1(x.data_ptr(), rows, cols, eps, em.data_ptr(), scale_idx, shift_idx, prev.data_ptr(), out.data_ptr(),
+                                            partials.data_ptr(), sums.data_ptr(), _stream()))
+    _count(2)
+    return out
+
+
 def colmean(x):
     """bf16 mean over the rows of a bf16 [rows, cols] view -> [1, cols] (torch semantics: bf16 sum, then bf16 division)."""
     _dev(x)

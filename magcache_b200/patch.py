@@ -20,7 +20,7 @@ import torch
 
 from . import ops
 from .config import FAMILIES, interp_cfg, nearest_interp, save_json, table_for_ckpt_dir, table_from_calibration, tables
-from .controller import AttrController, TeaController
+from .controller import AttrController, OpenSoraTeaController, TeaController, opensora_rel_l1
 from .mmdit import FluxEngine, FluxWeights, HunyuanEngine, HunyuanWeights
 from .opensora import OpenSoraEngine, OpenSoraWeights
 from .wan import WanEngine, WanWeights
@@ -533,6 +533,15 @@ def _opensora_unsupported(self, x_mask, kw):
         raise NotImplementedError("magcache_b200: Open-Sora with skip_y_embedder is not supported")
 
 
+def _opensora_stage(self, x, timestep, y, mask, x_mask, fps, height, width, kw):
+    _opensora_unsupported(self, x_mask, kw)
+    if not x.is_cuda:
+        raise RuntimeError("magcache_b200: x must be a CUDA tensor (no CPU path)")
+    eng = _cached_engine(self, "_mc_opensora_engine", lambda **skw: OpenSoraEngine(OpenSoraWeights.from_module(self, x.device), **skw))
+    eng.stage_inputs(x, timestep, y, mask, fps, height, width)
+    return eng
+
+
 def magcache_opensora_forward(self, x, timestep, all_timesteps, y, mask=None, x_mask=None, fps=None, height=None, width=None, **kw):
     r"""eval/magcache/experiments/opensora.py:229-373 on the H100 kernels (magcache_b200/opensora.py), with the same signature and
     class attributes (`t, skip_time, K, magcache_thresh, ratio, accumulated_sim / _err / _steps, skip_steps, residual_cache`).
@@ -541,11 +550,7 @@ def magcache_opensora_forward(self, x, timestep, all_timesteps, y, mask=None, x_
     reference's depth-3 FIFO is only ever read at [..., -1]; a tensor the caller puts there is honoured through its [..., -1].
     Cross-attention follows `flash_attn_varlen_func`: each sample attends to its own `y_lens[b]` caption tokens (the default
     `torch_impl` agrees whenever the lengths are equal, as for one prompt's CFG pair)."""
-    _opensora_unsupported(self, x_mask, kw)
-    if not x.is_cuda:
-        raise RuntimeError("magcache_b200: x must be a CUDA tensor (no CPU path)")
-    eng = _cached_engine(self, "_mc_opensora_engine", lambda **skw: OpenSoraEngine(OpenSoraWeights.from_module(self, x.device), **skw))
-    eng.stage_inputs(x, timestep, y, mask, fps, height, width)
+    eng = _opensora_stage(self, x, timestep, y, mask, x_mask, fps, height, width, kw)
     skip_forward = self.t >= self.skip_time and _ctrl(self, "opensora").decide(self)  # :297-308
     cur = self.residual_cache
     _take_residual(eng, cur[..., -1] if torch.is_tensor(cur) else cur)
@@ -572,6 +577,52 @@ def init_magcache_opensora(transformer, thresh=0.12, K=3, skip_time=6, ratio=Non
     cls.t, cls.residual_cache, cls.accumulated_err, cls.accumulated_sim, cls.accumulated_steps, cls.skip_steps = 0, None, 0, 1, 0, 0
     cls.cache_time = 4
     cls.ratio = np.asarray(tables()["opensora_eval"] if ratio is None else ratio, dtype=np.float64)
+    return transformer
+
+
+_TEA_OS = OpenSoraTeaController()
+
+
+def teacache_opensora_forward(self, x, timestep, all_timesteps, y, mask=None, x_mask=None, fps=None, height=None, width=None, **kw):
+    r"""`teacache_forward` of eval/magcache/experiments/opensora.py:34-227 (the paper's TeaCache arm for Open-Sora) on the H100 kernels,
+    with the same signature and class attributes (`enable_teacache, rel_l1_thresh, accumulated_rel_l1_distance,
+    previous_modulated_input, previous_residual`). The decision input is block 0's first LN + t2i_modulate of `x_embedder(x) + pos_emb`
+    over all samples; one fused kernel writes it and takes its relative L1 distance to the previous call's, and a miss feeds that
+    same tensor to block 0's qkv projection. A call is forced when `timestep[0]` (rounded to bf16) equals the first or the last of
+    `all_timesteps`; there is no counter and nothing is reset between videos. `previous_modulated_input` / `previous_residual` are
+    views of the engine's buffers, (B, N, C); a tensor the caller puts there is honoured. With `enable_teacache` False the call is the
+    plain forward (`eval_base`). Unsupported inputs raise as in `magcache_opensora_forward`."""
+    eng = _opensora_stage(self, x, timestep, y, mask, x_mask, fps, height, width, kw)
+    if not self.enable_teacache:  # :157-197
+        return eng.forward_plain()
+    eng.prologue("hit")  # x_embedder + pos_emb, t / fps / t_block; the caption MLP waits for the decision
+    ts = timestep.to(torch.bfloat16)  # `timestep = timestep.to(dtype)` (:51)
+    forced = bool(ts[0] == all_timesteps[0] or ts[0] == all_timesteps[-1])  # :96
+    eng.take_modulated_input(self.previous_modulated_input)
+    if not forced and eng.mi_prev is None:
+        raise TypeError("magcache_b200: TeaCache distance with no previous_modulated_input (reference: Tensor - NoneType)")
+    sums = eng.modulated_input(distance=not forced)
+    rel = None if forced else opensora_rel_l1(sums[0], sums[1], eng.R * eng.w.dim)
+    calc = _TEA_OS.decide(self, forced, rel)  # :96-107
+    self.previous_modulated_input = eng.mi[eng.mi_prev].view(eng.B, eng.N, -1)  # :108
+    if not calc:
+        cur = self.previous_residual
+        _take_residual(eng, cur.reshape(eng.res.shape) if torch.is_tensor(cur) else cur)
+    out = eng.forward_teacache(calc)
+    if calc:
+        self.previous_residual = eng.res.view(eng.B, eng.N, -1)  # :156
+    return out
+
+
+def init_teacache_opensora(transformer, rel_l1_thresh=0.1):
+    """The attribute block of `eval_teacache_slow` / `eval_teacache_fast` (opensora.py:389-394, :403-408): thresholds 0.1 / 0.2."""
+    cls = transformer.__class__
+    cls.enable_teacache = True
+    cls.rel_l1_thresh = rel_l1_thresh
+    cls.accumulated_rel_l1_distance = 0
+    cls.previous_modulated_input = None
+    cls.previous_residual = None
+    cls.forward = teacache_opensora_forward
     return transformer
 
 

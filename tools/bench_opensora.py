@@ -7,7 +7,13 @@ presets from their skip schedules, spatial-attention TFLOP/s, temporal-attention
 events in a separate profiled call), each next to the algorithmic figure computed here from the shapes, and the same forward through
 tests/opensora_ref.py in bf16 with torch SDPA (the reference's own path). The card, power limit and SM clock are read in the same run.
 
-    python tools/bench_opensora.py [--reps 3] [--frames 15]
+    python tools/bench_opensora.py [--reps 3] [--frames 15] [--teacache]
+
+--teacache adds TeaCache's hit and miss (`teacache_opensora_forward`'s engine path: decision input + distance, one host sync, then
+the residual add or the block stack), and the fused decision-input kernel (`mc_ln_t2i_modulate_rel_l1`, both samples) in µs and GB/s
+against its algorithmic bytes (x0 read, prev read, cur written), next to the unfused pair: `mc_ln_modulate` mode 2 followed by a
+separate distance pass (torch's `(cur - prev).abs().sum()` and `prev.abs().sum()`), against its algorithmic bytes (+ cur read back).
+No TeaCache seconds per video: with random weights its data-dependent hit count says nothing about the real model.
 """
 import argparse
 import json
@@ -42,11 +48,55 @@ def _time(fn, reps):
     return min(ts), sorted(ts)[len(ts) // 2]
 
 
+def _teacache(eng, reps, ops):
+    """TeaCache hit / miss ms and the decision-input kernel, fused and unfused, at the engine's staged shape."""
+    B, R, D = eng.B, eng.R, eng.w.dim
+    eng.prologue("hit")
+    eng.modulated_input(distance=False)  # a forced call: fills previous_modulated_input
+    eng.forward_teacache(True)
+
+    def call(calc):
+        eng.prologue("hit")
+        eng.modulated_input(distance=True)
+        eng.forward_teacache(calc)
+
+    call(False), call(True)
+    torch.cuda.synchronize()
+    tmiss = _time(lambda: call(True), reps)
+    thit = _time(lambda: call(False), reps)
+    prev, cur = eng.mi[eng.mi_prev], eng.mi[1 - eng.mi_prev]
+    em = [eng.modf[0, b].view(6, D) for b in range(B)]
+
+    def fused():
+        eng.tea_sums.zero_()
+        for b in range(B):
+            ops.ln_t2i_modulate_rel_l1(eng.x0[eng.rows(b)], em[b], 1, 0, prev[eng.rows(b)], cur[eng.rows(b)], eng.tea_partials, eng.tea_sums)
+
+    def unfused():
+        for b in range(B):
+            ops.ln_t2i_modulate(eng.x0[eng.rows(b)], em[b], 1, 0, out=cur[eng.rows(b)])
+        torch.stack([(cur - prev).abs().sum(dtype=torch.float32), prev.abs().sum(dtype=torch.float32)])
+
+    n = 200
+    out = {}
+    for name, fn, nbytes in (("fused", fused, 3 * R * D * 2), ("unfused", unfused, 4 * R * D * 2)):
+        for _ in range(10):
+            fn()
+        torch.cuda.synchronize()
+        best = min(_time(lambda: [fn() for _ in range(n)], 3)) / n  # ms per call pair
+        out[f"tea_input_{name}_us"] = round(best * 1e3, 1)
+        out[f"tea_input_{name}_mb"] = round(nbytes / 1e6, 1)
+        out[f"tea_input_{name}_gbps"] = round(nbytes / (best * 1e-3) / 1e9, 1)
+    return {"tea_miss_ms_min": round(tmiss[0], 2), "tea_miss_ms_median": round(tmiss[1], 2), "tea_hit_ms_min": round(thit[0], 2),
+            "tea_hit_ms_median": round(thit[1], 2), **out}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--frames", type=int, default=15)
     ap.add_argument("--skip-oracle", action="store_true")
+    ap.add_argument("--teacache", action="store_true")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_opensora needs a CUDA device")
@@ -104,6 +154,8 @@ def main():
             res[f"{preset}_hits"] = hits
             res[f"{preset}_s_per_video"] = round(((30 - hits) * miss[1] + hits * hit[1]) / 1e3, 2)
         res["no_cache_s_per_video"] = round(30 * miss[1] / 1e3, 2)
+        if a.teacache:
+            res.update(_teacache(eng, a.reps, ops))
         if not a.skip_oracle:
             R.install_magcache(model.__class__, thresh=0.0, K=0, skip_time=100)
             call = lambda: model(x, ts, None, y, mask=mask, fps=fps, height=hh, width=ww)  # noqa: E731
