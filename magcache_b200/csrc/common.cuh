@@ -90,17 +90,17 @@ __device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w 
 // torch.nn.GELU() (exact, erf form) in fp32: 0.5*x*(1+erf(x/sqrt(2))) — `img_emb` of the i2v models
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
-// torch.nn.GELU(approximate='tanh') in fp32: 0.5*x*(1+tanh(sqrt(2/pi)*(x+0.044715*x^3)))
+// torch.nn.GELU(approximate='tanh') in fp32, in the operation order of torch's CUDA kernel (ActivationGeluKernel.cu):
+// 0.5*x*(1+tanh(kBeta*(x+kKappa*x_cube))), x_cube = x*x*x, with an accurate tanhf. The old tanh.approx.f32 (MUFU.TANH) was
+// not good enough: for x < 0, t -> -1 and the output 0.5*x*(1+t) shrinks like exp(-x^2/2), so its error in t became up to
+// 13 596 bf16 ulps of the output (at x = -4.875). On every bf16 input this matches torch's F.gelu bit for bit, whether or not
+// `x + kKappa*x_cube` is contracted into an FMA; it is written with one rounding per op so that no compiler setting decides.
 __device__ __forceinline__ float gelu_tanh(float x) {
   const float kBeta = 0.7978845608028654f;  // sqrt(2/pi)
   const float kKappa = 0.044715f;
-  const float u = kBeta * (x + kKappa * x * x * x);
-  // one MUFU.TANH (tanh.approx.f32, |rel err| ~ 2^-11) instead of tanhf's ~20 instructions: the result is rounded to
-  // bf16 (2^-9 relative) by every caller, so the approximation is invisible after rounding except on exact ties
-  float t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(u));
-  const float hx = 0.5f * x;
-  return fmaf(hx, t, hx);
+  const float x3 = x * x * x;
+  const float inner = kBeta * __fadd_rn(x, __fmul_rn(kKappa, x3));
+  return 0.5f * x * (1.0f + tanhf(inner));
 }
 
 // RoPE in fp32 on four consecutive (real, imag) pairs, cs holding (cos, sin) per pair: every product and every sum rounded on
