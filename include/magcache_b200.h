@@ -278,7 +278,14 @@ int32_t mc_rmsnorm_head72_rope(void* x_bf16, int64_t ld, int64_t rows, int32_t h
 int32_t mc_attn_varlen_d72(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
                            int32_t heads, const int32_t* segs_dev, int32_t n_segs, int32_t max_q_len, float scale, void* stream);
 /* The temporal self-attention of STDiT3Block (open_sora_transformer_3d.py:196-198) without the `rearrange` copies: the rows of
- * q / k / v / out are in B (T S) C order, and sequence (b, s) is the T rows b*T*S + t*S + s, t < T <= 32. head_dim 72. */
+ * q / k / v / out are in B (T S) C order, and sequence (b, s) is the T rows b*T*S + t*S + s, t < T. head_dim 72. The kernel and
+ * its rounding chain follow from T:
+ *   T <= 32 (videos up to 4 s): attn_temporal_d72_kernel, P in fp32: fp32 dot products, e = exp2f(x - m), fp32 online softmax
+ *     and accumulation of e * v, out = bf16(acc / l). Only the output is rounded.
+ *   T > 32 (8 s and longer: T = 60, 120, 240): attn_temporal_mma_d72_kernel, the chain of mc_attn_varlen_d72: fp32 scores from
+ *     mma.sync, e = exp2f(x - m_tile) per 64-key tile, e rounded to bf16 for the PV product (fp32 accumulation), the row sum l
+ *     over the unrounded e, out = bf16(acc / l).
+ * Past 32 frames B*S*heads*ceil(T/64) must fit one grid dimension (< 2^31) and B*T*S < 2^31; otherwise MC_ERR_INVALID. */
 int32_t mc_attn_temporal_d72(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
                              int32_t B, int32_t T, int32_t S, int32_t heads, float scale, void* stream);
 

@@ -5,6 +5,9 @@
 //     caption lengths (OpenSoraMultiHeadCrossAttention.flash_attn_impl, attentions.py:136-153).
 //   * attn_temporal_d72_kernel: the temporal self-attention over B*S sequences of T <= 32 frames, read in place from the B (T S) C
 //     row order (the reference's `rearrange` copies around it, :196-198, are not made).
+//   * attn_temporal_mma_d72_kernel: the same attention for T > 32 (8 s videos and longer: T = 60, 120, 240), on the varlen kernel's
+//     tensor-core tile with strided rows. Both instantiations share one tile body; the row addressing (segment table and unit
+//     stride, or sequence from the grid and stride S) is a compile-time policy.
 //   * rmsnorm_head72_rope_kernel: the q / k LlamaRMSNorm(72) and the temporal RoPE (attentions.py:71-75).
 //
 // The varlen kernel is a separate mma.sync (m16n8k16) kernel rather than a head_dim template of attn_kernel, so that attn_kernel's
@@ -56,33 +59,41 @@ __device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], 
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-// rows [row0, row0 + 64) of one head (72 columns) -> shared [64][kLd]; rows at or past `n` are zero-filled
-__device__ __forceinline__ void load_tile(__nv_bfloat16* dst, const __nv_bfloat16* src, int64_t ld, int64_t row0, int n, int tid) {
+// Row addressing of a query or key range: element r of the range that starts at row `row0`. The varlen segments are contiguous
+// row ranges; a temporal sequence (b, s) has its frames S rows apart (frame t at row b*T*S + t*S + s).
+struct UnitRows {
+  __device__ __forceinline__ int64_t operator()(int64_t row0, int r) const { return row0 + r; }
+};
+struct StridedRows {
+  int64_t stride;
+  __device__ __forceinline__ int64_t operator()(int64_t row0, int r) const { return row0 + r * stride; }
+};
+
+// range elements [0, 64) starting at row0 of one head (72 columns) -> shared [64][kLd]; elements at or past `n` are zero-filled
+template <class Rows>
+__device__ __forceinline__ void load_tile(__nv_bfloat16* dst, const __nv_bfloat16* src, int64_t ld, int64_t row0, int n, int tid, Rows rows) {
   for (int i = tid; i < kBK * 9; i += kThreads) {
     const int r = i / 9, c = i - r * 9;
     const bool ok = r < n;
-    cp_async16(dst + r * kLd + c * 8, ok ? src + (row0 + r) * ld + c * 8 : src, ok);
+    cp_async16(dst + r * kLd + c * 8, ok ? src + rows(row0, r) * ld + c * 8 : src, ok);
   }
 }
 
 }  // namespace os
 
-// segs: int32 [n_seg, 4] = (q_start, q_len, k_start, k_len). grid (q tiles of the longest segment, n_seg, heads).
-__global__ void __launch_bounds__(os::kThreads) attn_varlen_d72_kernel(const __nv_bfloat16* __restrict__ q, int64_t ldq,
-                                                                       const __nv_bfloat16* __restrict__ k, int64_t ldk,
-                                                                       const __nv_bfloat16* __restrict__ v, int64_t ldv,
-                                                                       __nv_bfloat16* __restrict__ out, int64_t ldo,
-                                                                       const int32_t* __restrict__ segs, float scale_log2) {
+// One CTA: query elements [q0, q0 + 64) of the q range (q_start, q_len) of head h against the whole k / v range (k_start,
+// k_len), k_len >= 1, q0 < q_len. mma.sync m16n8k16, 64-key tiles double-buffered with cp.async, online softmax in base 2; P is
+// rounded to bf16 for the PV product, the row sum l is taken over the unrounded P.
+template <class Rows>
+__device__ __forceinline__ void attn_d72_tile(const __nv_bfloat16* __restrict__ q, int64_t ldq, const __nv_bfloat16* __restrict__ k,
+                                              int64_t ldk, const __nv_bfloat16* __restrict__ v, int64_t ldv,
+                                              __nv_bfloat16* __restrict__ out, int64_t ldo, int q_start, int q_len, int k_start,
+                                              int k_len, int q0, int h, float scale_log2, Rows rows) {
   using namespace os;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(smem_raw);
   __nv_bfloat16* sKV = sQ + kBQ * kLd;  // stage s: K at sKV + (2s) * kTileElems, V at sKV + (2s+1) * kTileElems
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int4 sg = reinterpret_cast<const int4*>(segs)[blockIdx.y];
-  const int q_start = sg.x, q_len = sg.y, k_start = sg.z, k_len = sg.w;
-  const int q0 = blockIdx.x * kBQ;
-  if (q0 >= q_len || k_len <= 0) return;
-  const int h = blockIdx.z;
   const __nv_bfloat16* qh = q + h * kD;
   const __nv_bfloat16* kh = k + h * kD;
   const __nv_bfloat16* vh = v + h * kD;
@@ -93,9 +104,9 @@ __global__ void __launch_bounds__(os::kThreads) attn_varlen_d72_kernel(const __n
     *reinterpret_cast<uint4*>(row + kD) = make_uint4(0u, 0u, 0u, 0u);
   }
   const int n_tiles = (k_len + kBK - 1) / kBK;
-  load_tile(sQ, qh, ldq, static_cast<int64_t>(q_start) + q0, q_len - q0, tid);
-  load_tile(sKV, kh, ldk, k_start, k_len, tid);
-  load_tile(sKV + kTileElems, vh, ldv, k_start, k_len, tid);
+  load_tile(sQ, qh, ldq, rows(q_start, q0), q_len - q0, tid, rows);
+  load_tile(sKV, kh, ldk, k_start, k_len, tid, rows);
+  load_tile(sKV + kTileElems, vh, ldv, k_start, k_len, tid, rows);
   cp_async_commit();
 
   uint32_t qf[5][4];
@@ -108,8 +119,8 @@ __global__ void __launch_bounds__(os::kThreads) attn_varlen_d72_kernel(const __n
     if (t + 1 < n_tiles) {
       const int st = (t + 1) & 1;
       const int kr = (t + 1) * kBK;
-      load_tile(sKV + (2 * st) * kTileElems, kh, ldk, static_cast<int64_t>(k_start) + kr, k_len - kr, tid);
-      load_tile(sKV + (2 * st + 1) * kTileElems, vh, ldv, static_cast<int64_t>(k_start) + kr, k_len - kr, tid);
+      load_tile(sKV + (2 * st) * kTileElems, kh, ldk, rows(k_start, kr), k_len - kr, tid, rows);
+      load_tile(sKV + (2 * st + 1) * kTileElems, vh, ldv, rows(k_start, kr), k_len - kr, tid, rows);
       cp_async_commit();
       cp_async_wait<1>();
     } else {
@@ -199,10 +210,41 @@ __global__ void __launch_bounds__(os::kThreads) attn_varlen_d72_kernel(const __n
 #pragma unroll
   for (int j = 0; j < 9; ++j) {
     if (r0 < q_len)
-      *reinterpret_cast<uint32_t*>(oh + (static_cast<int64_t>(q_start) + r0) * ldo + j * 8) = pack_bf16x2(o[j][0] * i0, o[j][1] * i0);
+      *reinterpret_cast<uint32_t*>(oh + rows(q_start, r0) * ldo + j * 8) = pack_bf16x2(o[j][0] * i0, o[j][1] * i0);
     if (r1 < q_len)
-      *reinterpret_cast<uint32_t*>(oh + (static_cast<int64_t>(q_start) + r1) * ldo + j * 8) = pack_bf16x2(o[j][2] * i1, o[j][3] * i1);
+      *reinterpret_cast<uint32_t*>(oh + rows(q_start, r1) * ldo + j * 8) = pack_bf16x2(o[j][2] * i1, o[j][3] * i1);
   }
+}
+
+// segs: int32 [n_seg, 4] = (q_start, q_len, k_start, k_len). grid (q tiles of the longest segment, n_seg, heads).
+__global__ void __launch_bounds__(os::kThreads) attn_varlen_d72_kernel(const __nv_bfloat16* __restrict__ q, int64_t ldq,
+                                                                       const __nv_bfloat16* __restrict__ k, int64_t ldk,
+                                                                       const __nv_bfloat16* __restrict__ v, int64_t ldv,
+                                                                       __nv_bfloat16* __restrict__ out, int64_t ldo,
+                                                                       const int32_t* __restrict__ segs, float scale_log2) {
+  const int4 sg = reinterpret_cast<const int4*>(segs)[blockIdx.y];
+  const int q_start = sg.x, q_len = sg.y, k_start = sg.z, k_len = sg.w;
+  const int q0 = blockIdx.x * os::kBQ;
+  if (q0 >= q_len || k_len <= 0) return;
+  attn_d72_tile(q, ldq, k, ldk, v, ldv, out, ldo, q_start, q_len, k_start, k_len, q0, blockIdx.z, scale_log2, os::UnitRows{});
+}
+
+// Temporal attention for T > kTempMaxT on the tensor cores: the varlen kernel's tile with the frames of sequence (b, s) as both the
+// query and the key range (frame t at row b*T*S + t*S + s), no segment table. One flat grid dimension, q tile fastest, then head,
+// then sequence, so the CTAs that share a sequence's K / V run together and neighbouring sequences read neighbouring rows.
+__global__ void __launch_bounds__(os::kThreads) attn_temporal_mma_d72_kernel(const __nv_bfloat16* __restrict__ q, int64_t ldq,
+                                                                             const __nv_bfloat16* __restrict__ k, int64_t ldk,
+                                                                             const __nv_bfloat16* __restrict__ v, int64_t ldv,
+                                                                             __nv_bfloat16* __restrict__ out, int64_t ldo, int T, int S,
+                                                                             int heads, float scale_log2) {
+  const unsigned q_tiles = (T + os::kBQ - 1) / os::kBQ;
+  const unsigned x = blockIdx.x / q_tiles;
+  const int q0 = static_cast<int>(blockIdx.x - x * q_tiles) * os::kBQ;
+  const unsigned seq = x / heads;  // b * S + s
+  const int h = static_cast<int>(x - seq * heads);
+  const unsigned b = seq / S, s = seq - b * S;
+  const int row0 = static_cast<int>(b * T * S + s);  // B*T*S < 2^31 (checked at launch)
+  attn_d72_tile(q, ldq, k, ldk, v, ldv, out, ldo, row0, T, row0, T, q0, h, scale_log2, os::StridedRows{S});
 }
 
 // Temporal attention: one warp per (sequence b*S + s, head), lane = query frame. The T key / value rows of the sequence (S rows
@@ -345,11 +387,25 @@ int32_t mc_attn_varlen_d72(const void* q, int64_t ldq, const void* k, int64_t ld
 int32_t mc_attn_temporal_d72(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out, int64_t ldo,
                              int32_t B, int32_t T, int32_t S, int32_t heads, float scale, void* stream) {
   MC_CHECK_ARG(q && k && v && out, "mc_attn_temporal_d72: null pointer");
-  MC_CHECK_ARG(B >= 1 && S >= 1 && T >= 1 && T <= mc::kTempMaxT && heads >= 1, "mc_attn_temporal_d72: B=%d T=%d S=%d heads=%d (T <= 32)", B, T, S, heads);
+  MC_CHECK_ARG(B >= 1 && S >= 1 && T >= 1 && heads >= 1, "mc_attn_temporal_d72: B=%d T=%d S=%d heads=%d", B, T, S, heads);
   MC_CHECK_ARG(static_cast<int64_t>(B) * S <= 0x7fffffff, "mc_attn_temporal_d72: B*S too large");
   MC_CHECK_ARG(ld_ok(ldq, heads) && ld_ok(ldk, heads) && ld_ok(ldv, heads) && ld_ok(ldo, heads),
                "mc_attn_temporal_d72: leading dimensions must be multiples of 8 and >= heads*72");
   MC_CHECK_ARG(mc::aligned16(q) && mc::aligned16(k) && mc::aligned16(v) && mc::aligned16(out), "mc_attn_temporal_d72: pointers must be 16-byte aligned");
+  if (T > mc::kTempMaxT) {
+    const int64_t q_tiles = (T + mc::os::kBQ - 1) / mc::os::kBQ;
+    const int64_t ctas = static_cast<int64_t>(B) * S * heads * q_tiles;
+    MC_CHECK_ARG(static_cast<int64_t>(B) * T * S <= 0x7fffffff, "mc_attn_temporal_d72: B*T*S rows exceed int32");
+    MC_CHECK_ARG(ctas <= 0x7fffffff,"mc_attn_temporal_d72: B*S*heads*ceil(T/64) = %lld CTAs exceed one grid dimension", static_cast<long long>(ctas));
+    static mc::PerDeviceOnce once;
+    int32_t rc = mc::set_max_smem_once(mc::attn_temporal_mma_d72_kernel, mc::os::kSmemBytes, once, "cudaFuncSetAttribute(attn_temporal_mma_d72 smem)");
+    if (rc) return rc;
+    mc::attn_temporal_mma_d72_kernel<<<static_cast<unsigned>(ctas), mc::os::kThreads, mc::os::kSmemBytes, static_cast<cudaStream_t>(stream)>>>(
+        static_cast<const __nv_bfloat16*>(q), ldq, static_cast<const __nv_bfloat16*>(k), ldk, static_cast<const __nv_bfloat16*>(v), ldv,
+        static_cast<__nv_bfloat16*>(out), ldo, T, S, heads, scale * 1.4426950408889634f);
+    MC_CHECK_LAUNCH("attn_temporal_mma_d72_kernel launch");
+    return MC_OK;
+  }
   const dim3 grid(static_cast<unsigned>(static_cast<int64_t>(B) * S), (heads + mc::kTempWarps - 1) / mc::kTempWarps);
   mc::attn_temporal_d72_kernel<<<grid, mc::kTempWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(q), ldq, static_cast<const __nv_bfloat16*>(k), ldk, static_cast<const __nv_bfloat16*>(v), ldv,

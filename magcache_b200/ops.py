@@ -301,7 +301,9 @@ def attention_varlen_d72(q, k, v, heads, segs, max_q_len, scale=None, out=None, 
 
 
 def attention_temporal_d72(q, k, v, heads, B, T, S, scale=None, out=None, tag=None):
-    """Temporal attention (`mc_attn_temporal_d72`): rows in B (T S) C order, sequence (b, s) = rows b*T*S + t*S + s; head_dim 72."""
+    """Temporal attention (`mc_attn_temporal_d72`): rows in B (T S) C order, sequence (b, s) = rows b*T*S + t*S + s; head_dim 72.
+    T <= 32 keeps P in fp32 (one lane per query frame); T > 32 runs on the tensor cores and rounds P to bf16 for the PV product,
+    as `attention_varlen_d72` does. The kernel is chosen from T alone."""
     _dev(q), _dev(k), _dev(v)
     for t_ in (q, k, v):
         assert t_.dtype == torch.bfloat16 and t_.stride(1) == 1 and t_.shape == (B * T * S, heads * 72)

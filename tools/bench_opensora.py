@@ -3,9 +3,11 @@
 Workload: the default of OpenSoraPipeline.generate under the paper's eval settings — 480p 9:16 (480 x 854 -> a 60 x 106 latent,
 30 x 53 = 1590 patches per frame), 51 frames (T = 15 latent frames), B = 2 (the CFG pair), 300 caption tokens, 30 sampling steps,
 full-size seeded random weights. Prints one JSON line: miss / hit forward ms (CUDA events), seconds per 30-step video for both paper
-presets from their skip schedules, spatial-attention TFLOP/s, temporal-attention GB/s and the GEMMs' share of a miss (from per-launch
-events in a separate profiled call), each next to the algorithmic figure computed here from the shapes, and the same forward through
-tests/opensora_ref.py in bf16 with torch SDPA (the reference's own path). The card, power limit and SM clock are read in the same run.
+presets from their skip schedules, spatial-attention TFLOP/s, temporal-attention GB/s and TFLOP/s and the GEMMs' share of a miss
+(from per-launch events in a separate profiled call), each next to the algorithmic figure computed here from the shapes, and the same
+forward through tests/opensora_ref.py in bf16 with torch SDPA (the reference's own path). The card, power limit and SM clock are read
+in the same run. --frames sets T, the latent frames: 15, 30, 60, 120, 240 for the 2, 4, 8, 16, 32 s videos; past 32 frames the
+temporal attention runs on the tensor cores (attn_temporal_mma_d72_kernel), up to 32 on the CUDA cores.
 
     python tools/bench_opensora.py [--reps 3] [--frames 15] [--teacache]
 
@@ -147,6 +149,7 @@ def main():
                "cross_attn_tflop_per_launch": round(cr_flops / 1e12, 3),
                "temporal_attn_gflop_per_launch": round(tp_flops / 1e9, 2), "temporal_attn_mb_per_launch": round(tp_bytes / 1e6, 1),
                "temporal_attn_ms": round(tp_ms, 3), "temporal_attn_gbps": round(tp_bytes / tp_ms / 1e6, 1) if tp_ms else None,
+               "temporal_attn_tflops": round(tp_flops / tp_ms / 1e9, 1) if tp_ms else None,
                "launch_ms_by_tag": {k: round(v, 2) for k, v in sorted(prof.items(), key=lambda kv: -kv[1])}}
         for preset in ("opensora-slow-E012K3", "opensora-fast-E024K5"):
             m = mc.PRESETS[preset].schedule()
