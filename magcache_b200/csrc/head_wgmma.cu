@@ -46,9 +46,9 @@ struct Layout {
   static constexpr int kRawStages = HIT ? 2 : 3;                    // 96 KB of loads in flight per SM either way
   static constexpr int kOffRaw = kOpStages * kOpStage;              // 96 KB
   static constexpr int kOffStats = kOffRaw + kRawStages * kRawStage;  // 192 KB
-  static constexpr int kOffAcc = kOffStats + kRows * 8;
+  static constexpr int kOffAcc = kOffStats + 2 * kRows * 8;          // row statistics, double-buffered by row tile
   static constexpr int kOffBars = kOffAcc + kRows * kAccPad * 4;
-  static constexpr int kSmem = kOffBars + 256;      // 231168 of the 232448 an H100 block may use
+  static constexpr int kSmem = kOffBars + 256;      // 232192 of the 232448 an H100 block may use
 };
 }  // namespace hd
 
@@ -137,7 +137,10 @@ __global__ void __launch_bounds__(hd::kThreads, 1) head_tc_kernel(const __grid_c
   using namespace hd;
   using L = Layout<HIT>;
   extern __shared__ __align__(1024) uint8_t smem[];
-  float2* stats = reinterpret_cast<float2*>(smem + L::kOffStats);  // (mean - pilot, rstd) per tile row
+  // (mean - pilot, rstd) per tile row, [2][kRows]: tile st uses half st & 1. A converter warp publishes tile st + 1's statistics
+  // before the barrier of tile st + 1, while an epilogue warp may still read tile st's: with one or two chunks per row (cols <=
+  // 128) nothing else holds the converter back. It cannot reach tile st + 2 before every epilogue warp has passed that barrier.
+  float2* stats_buf = reinterpret_cast<float2*>(smem + L::kOffStats);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kOffBars);
   uint64_t* raw_full = bars + 0;    // [kRawStages] TMA
   uint64_t* raw_empty = bars + 3;   // [kRawStages] 16 arrivals (one per converter warp): the raw chunk has been read into registers
@@ -226,6 +229,7 @@ __global__ void __launch_bounds__(hd::kThreads, 1) head_tc_kernel(const __grid_c
     const float inv_cols = 1.0f / static_cast<float>(p.cols);
     for (int st = 0; st < n_sub; ++st) {
       int prev_os = -1;
+      float2* stats = stats_buf + (st & 1) * kRows;
       const int64_t row = cta_row0 + static_cast<int64_t>(st) * kRows + rt;
       const bool live = row < cta_row1;
       float pilot = 0.f, mean = 0.f, m2 = 0.f;  // running mean / M2 of the shifted values over the slices this thread has seen

@@ -5,7 +5,10 @@ the bytes feed a stored result writes NaN; output margins hold a fixed byte patt
 the call, so a store past a row or past a tensor fails the test instead of landing in allocator slack. The shapes are the ragged
 tiles, the wholly out-of-range half tiles, the idle warps and the unaligned tails: K not a multiple of 64 and N = 32 in the GEMM
 (Open-Sora's x_embedder and final layer), an 11-key attention (HunyuanVideo's token refiner), key views of longer buffers,
-segments of 1 / 63 / 64 / 65 rows, and the like. Results are compared with fp64 statements of each kernel's rounding chain, at
+segments of 1 / 63 / 64 / 65 rows, and the like. The staged row kernels, whose copy sizes are worked out at run time, are
+here too: LayerNorm + modulation (K7) and RMSNorm + RoPE (K9) either side of the 1024-row switch to the staging ring, with a
+ragged last stage, at every per-lane group count and the wide forms, and the residual statistics (K3) with a ragged last chunk
+of 4 rows and the fused residual output fenced. Results are compared with fp64 statements of each kernel's rounding chain, at
 the criteria of test_kernels_gpu.py and test_opensora_gpu.py; where a result is exact (one key, a 30-logit peak, the
 elementwise kernels) it is compared bit for bit.
 
@@ -669,3 +672,166 @@ def test_cfg_kernels_and_dequant_fenced():
         ops.dequant_fp8_bf16(q, sc, o.view(rows, cols))
         check_fence(o, obuf)
         assert torch.equal(o.view(rows, cols), q.to(BF) * sc[:, None]), (rows, cols)
+
+
+# ------------------------------------------------------------------------------------------- staged row kernels (K7, K9, K3)
+U32 = 2.0 ** -24  # fp32 unit roundoff
+
+
+def _staged_rows(sms):
+    """Row counts either side of the 1024-row switch to the staged forms, a ragged last chunk of 8, and two chunks per CTA
+    plus a ragged one."""
+    return (1023, 1024, 1025, 1031, 2 * 8 * sms + 3)
+
+
+def _ln_chain(x, a, b, mode, round_ln, out_bf16, eps=1e-6):
+    """fp64 reference and per-element bound of K7 (`mc_ln_modulate` modes 0 / 1) on x [rows, cols]: y = LN(x) (rounded to bf16
+    when round_ln) times aa = fp32(1 + a) (mode 0) or a (mode 1), plus b, each rounded in fp32, stored as bf16 or fp32.
+    The fp32 two-pass statistics: a lane sums at most cols / 32 values and the warp (or team) adds 5-7 levels, so the mean is
+    within (cols / 32 + 8) u mean|x| and the variance relative within (cols / 32 + 10) u, plus the mean error squared; rsqrtf
+    2 ulp, (x - mean) * rstd 2 u. round_ln may flip the LN value's bf16 rounding by one ulp (2^-7 relative); the bf16 store
+    adds half an ulp (2^-8)."""
+    v = x.double()
+    cols = v.shape[1]
+    k = cols / 32 + 8
+    mu = v.mean(1, keepdim=True)
+    var = (v - mu).pow(2).mean(1, keepdim=True)
+    rstd = (var + eps).rsqrt()
+    ln = (v - mu) * rstd
+    dmu = k * U32 * v.abs().mean(1, keepdim=True)
+    e_r = 0.5 * ((k + 2) * U32 + dmu.pow(2) / (var + eps)) + 3 * U32
+    e_ln = dmu * rstd + (e_r + 2 * U32) * ln.abs()
+    aa = ((1.0 + a) if mode == 0 else a).double()  # fp32 1 + a, as the kernel forms it
+    if round_ln:
+        ln = _rb(ln)
+        e_ln = e_ln + ln.abs() * 2.0 ** -7
+    ref = ln * aa + b.double()
+    bound = e_ln * aa.abs() + U32 * (2 * (ln * aa).abs() + ref.abs())
+    if out_bf16:
+        bound = bound * (1 + 2.0 ** -8) + ref.abs() * 2.0 ** -8
+    return ref, bound
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("cols", [256, 384, 1024, 1536, 2048, 3072, 5120])
+def test_ln_modulate_staged_fenced(cols):
+    """K7 (`mc_ln_modulate` modes 0 and 1) at the row counts either side of the staged form (G = 2 / 2 / 4 / 6 / 8 by width,
+    the wide team-per-row form at 3072 and 5120): x fp32 and bf16 with NaN rows after it, out fp32 and bf16 a row window of a
+    fenced buffer, round_ln on and off; every element against fp64 within `_ln_chain`'s bound."""
+    L = _lib()
+    ops = _ops()
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    g = torch.Generator(device=DEV).manual_seed(cols)
+    for rows in _staged_rows(sms):
+        for xdt in (F32, BF):
+            x, _ = fenced((rows, cols), xdt, (0, 8, 0, 0), pitch=cols)
+            x.copy_(_randn((rows, cols), g, 3.0) + 0.5)
+            p, _ = fenced((6 * cols,), F32, (0, 0, 8, 8))
+            p.copy_(_randn((6 * cols,), g, 0.3))
+            em = p.view(6, cols)
+            for mode in (0, 1):
+                a, b = (em[4], em[3]) if mode == 0 else (em[0], em[5])
+                for round_ln in (0, 1):
+                    for odt in (F32, BF):
+                        out, obuf = fenced((rows, cols), odt, (2, 2, 0, 0), fill="fence", pitch=cols)
+                        p0, p1 = (em, None) if mode == 0 else (em[0], em[5])
+                        L.check(L.lib.mc_ln_modulate(x.data_ptr(), L.MC_BF16 if xdt == BF else L.MC_F32, rows, cols, 1e-6, mode,
+                                                     p0.data_ptr(), None if p1 is None else p1.data_ptr(), 4, 3, round_ln,
+                                                     out.data_ptr(), L.MC_BF16 if odt == BF else L.MC_F32, ops._stream()))
+                        check_fence(out, obuf)
+                        ref, bound = _ln_chain(x, a, b, mode, round_ln, odt == BF)
+                        err = (out.double() - ref).abs()
+                        what = (rows, cols, xdt, mode, round_ln, odt)
+                        assert bool(torch.isfinite(out.float()).all()), what
+                        assert bool((err <= bound).all()), (what, float((err / bound).max()))
+
+
+def _rope64(o, cs, cols):
+    """fp64 RoPE of o [rows, cols] with cos_sin [rows, head_dim] (interleaved cos, sin): column c at position c % head_dim."""
+    hd = cs.shape[1]
+    c = cs.double()[:, torch.arange(cols, device=cs.device) % hd].reshape(o.shape[0], cols // 2, 2)
+    re, im = o.reshape(o.shape[0], cols // 2, 2).unbind(-1)
+    return torch.stack([re * c[..., 0] - im * c[..., 1], im * c[..., 0] + re * c[..., 1]], -1).reshape(o.shape)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("segs,rows", [(1, 1031), (2, 515), (4, 257), (3, 401), (1, 33), (2, 33)])
+@pytest.mark.parametrize("rope", [False, True])
+def test_rmsnorm_rope_segs_fenced(segs, rows, rope):
+    """K9 (`mc_rmsnorm_rope_segs`) in place on a strided view: segs 1 / 2 / 4 take the staged ring (ragged last stage), 3 the
+    register form; the fenced columns left of the view, between segs * cols and ld, right of it, and the fenced rows above and
+    below must keep their bytes; cos_sin has NaN rows after the last. cols 256 / 1024 / 1536 / 2048, and 5120 (one wide launch per
+    segment) at 33 rows. Every element of every segment within test_rmsnorm72_rope's ulp criterion of fp64."""
+    ops = _ops()
+    g = torch.Generator(device=DEV).manual_seed(segs * 1000 + rows + rope)
+    for cols in ((5120,) if rows == 33 else (256, 1024, 1536, 2048)):
+        x, xbuf = fenced((rows, segs * cols), BF, (1, 1, 8, 16), fill="fence")
+        x.copy_(_randn(x.shape, g, 2.0))
+        x0 = x.clone()
+        w, _ = fenced((segs * cols,), F32, (0, 0, 8, 8))
+        w.copy_(1 + 0.2 * _randn((segs * cols,), g))
+        cs = None
+        if rope:
+            cs, _ = fenced((rows, 128), F32, (0, 8, 0, 0), pitch=128)
+            cs.copy_(_rope_table(rows, 128, g))
+        ops.rmsnorm_rope_segs_(x, w.view(segs, cols), segs, cs, 128)
+        check_fence(x, xbuf)
+        for sg in range(segs):
+            v = x0[:, sg * cols:(sg + 1) * cols].double()
+            o = _rb(v * torch.rsqrt(v.pow(2).mean(-1, keepdim=True) + 1e-6)) * w[sg * cols:(sg + 1) * cols].double()
+            if rope:
+                o = _rope64(o, cs, cols)
+            _assert_ulps(x[:, sg * cols:(sg + 1) * cols], _rb(o), rope, (segs, rows, cols, sg, rope))
+
+
+def _stats_chain(c, p, eps=0.0):
+    """fp64 (sum ratio, sum ratio^2, sum (1 - cos)) over the rows of c, p and a bound from the per-row fp32 sums: each of
+    |c|^2, |p|^2, c.p is a fused multiply-add chain of cols / 32 terms per lane plus 5 shuffle levels, within
+    g = (cols / 32 + 6) u of the sum of |terms|; the norms (sqrtf), the ratio and the cosine add a few u."""
+    c, p = c.double(), p.double()
+    cols = c.shape[1]
+    gm = (cols / 32 + 6) * U32
+    nc, np_ = c.norm(dim=1), p.norm(dim=1)
+    dot = (c * p).sum(1)
+    ratio = nc / (np_ + eps)
+    cosv = dot / (nc.clamp_min(1e-8) * np_.clamp_min(1e-8))
+    e_ratio = ratio * (gm + 4 * U32)
+    e_cos = gm * (c * p).abs().sum(1) / (nc.clamp_min(1e-8) * np_.clamp_min(1e-8)) + cosv.abs() * (gm + 4 * U32) + U32
+    ref = torch.stack([ratio.sum(), ratio.pow(2).sum(), (1 - cosv).sum()])
+    bound = torch.stack([e_ratio.sum(), (2 * ratio * e_ratio + U32 * ratio.pow(2)).sum(), e_cos.sum()]) + 1e-12 * ref.abs()
+    return ref, bound
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("cols,dt", [(1536, F32), (3072, F32), (5120, F32), (1536, BF)])
+def test_residual_stats_fenced(cols, dt):
+    """K3 (`mc_residual_stats`, and `mc_residual_sub_stats` in fp32) at 1 / 3 / 4 / 5 / 1027 rows: fp32 1536 and 3072 take the
+    staged form (3072: two stages of 4 rows, the fused form the warp-per-row kernel), 5120 and bf16 the warp-per-row kernel;
+    inputs with NaN rows after them; the fused r_out a fenced row window, bit-equal to x_out - x_in; the three sums against
+    fp64 within `_stats_chain`'s bound."""
+    ops, L = _ops(), _lib()
+    g = torch.Generator(device=DEV).manual_seed(cols + (dt == BF))
+    code = L.MC_BF16 if dt == BF else L.MC_F32
+    for rows in (1, 3, 4, 5, 1027):
+        prev, _ = fenced((rows, cols), dt, (0, 8, 0, 0), pitch=cols)
+        prev.copy_(_randn((rows, cols), g, 0.1))
+        cur, _ = fenced((rows, cols), dt, (0, 8, 0, 0), pitch=cols)
+        cur.copy_(prev.float() * (0.97 + 0.05 * torch.rand(rows, 1, device=DEV, generator=g)) + _randn((rows, cols), g, 0.01))
+        stats = torch.empty(4, dtype=torch.float64, device=DEV)
+        L.check(L.lib.mc_residual_stats(cur.data_ptr(), code, prev.data_ptr(), code, rows, cols, 0.0, stats.data_ptr(), ops._stream()))
+        ref, bound = _stats_chain(cur, prev)
+        assert float(stats[3]) == rows
+        assert bool(((stats[:3] - ref).abs() <= bound).all()), (rows, cols, dt, stats.tolist(), ref.tolist())
+        if dt == BF:
+            continue
+        x_in, _ = fenced((rows, cols), BF, (0, 8, 0, 0), pitch=cols)
+        x_in.copy_(_randn((rows, cols), g))
+        x_out, _ = fenced((rows, cols), F32, (0, 8, 0, 0), pitch=cols)
+        x_out.copy_(x_in.float() + cur)
+        r, rbuf = fenced((rows, cols), F32, (1, 1, 0, 0), fill="fence", pitch=cols)
+        L.check(L.lib.mc_residual_sub_stats(x_out.data_ptr(), L.MC_F32, x_in.data_ptr(), L.MC_BF16, r.data_ptr(), prev.data_ptr(), rows,
+                                            cols, 0.0, stats.data_ptr(), ops._stream()))
+        check_fence(r, rbuf)
+        assert torch.equal(r, x_out - x_in.float()), (rows, cols)
+        ref, bound = _stats_chain(r, prev)
+        assert bool(((stats[:3] - ref).abs() <= bound).all()), (rows, cols, "fused", stats.tolist(), ref.tolist())

@@ -240,7 +240,9 @@ def test_patchify_matches_conv3d_im2col():
 @pytest.mark.parametrize("rows,cols,xdt", [(37, 1536, torch.float32), (130, 5120, torch.float32), (64, 1536, torch.bfloat16), (5, 256, torch.float32),
                                            # >= 1024 rows: the TMA-staged form (ragged last group of 8 rows, 2-8 ring stages)
                                            (1029, 1536, torch.float32), (4099, 1536, torch.bfloat16), (2050, 384, torch.float32),
-                                           (1500, 2048, torch.float32), (1025, 3072, torch.float32)])
+                                           (1500, 2048, torch.float32), (1025, 3072, torch.float32),
+                                           # cols 1024: four groups per lane (G = 4), the register and the staged form
+                                           (300, 1024, torch.bfloat16), (1029, 1024, torch.float32)])
 def test_ln_modulate(rows, cols, xdt):
     ops = _ops()
     x = (torch.randn(rows, cols, device=DEV) * 3 + 0.5).to(xdt)
@@ -557,31 +559,32 @@ def test_rmsnorm_rope_two_blocks_one_launch(rows, D):
 def test_rmsnorm_rope_staged_form_matches_register_form_bitwise():
     """The TMA-staged kernels (>= 1024 items) and the register-pipelined ones (fewer) run the same per-row arithmetic: the first
     1000 rows of a long input, processed alone, must come out bit-identical; likewise LayerNorm + modulation (mode 0) and the
-    affine LayerNorm (mode 1), from fp32 and from bf16 input with the LN value rounded to bf16, into bf16 and into fp32."""
+    affine LayerNorm (mode 1), from fp32 and from bf16 input with the LN value rounded to bf16, into bf16 and into fp32. The widths
+    D = 256 / 1024 / 1536 / 2048 cover every per-lane group count G = 2 / 4 / 6 / 8 of both kernels."""
     ops = _ops()
-    g = torch.Generator(device=DEV).manual_seed(3)
-    D = 1536
-    qkv = torch.randn(2500, 3 * D, device=DEV, generator=g).bfloat16()
-    w = 1 + 0.1 * torch.randn(2, D, device=DEV, generator=g)
-    cs = torch.randn(2500, 128, device=DEV, generator=g)
-    a, b = qkv.clone(), qkv[:500].clone()
-    ops.rmsnorm_rope_segs_(a, w, 2, cs, 128)         # 5000 items: staged
-    ops.rmsnorm_rope_segs_(b, w, 2, cs[:500], 128)   # 1000 items: register form
-    assert torch.equal(a[:500], b)
-    x = torch.randn(2500, D, device=DEV, generator=g) * 2 + 0.3
-    em = torch.randn(6, D, device=DEV, generator=g) * 0.2
-    ya = ops.ln_modulate(x, em, 4, 3)
-    yb = ops.ln_modulate(x[:1000], em, 4, 3)
-    assert torch.equal(ya[:1000], yb)
-    xh = x.bfloat16()
-    for out_dtype in (torch.bfloat16, torch.float32):
-        ya = ops.ln_modulate(xh, em, 1, 0, round_ln_to_bf16=True, out_dtype=out_dtype)
-        yb = ops.ln_modulate(xh[:1000], em, 1, 0, round_ln_to_bf16=True, out_dtype=out_dtype)
-        assert ya.dtype == out_dtype and torch.equal(ya[:1000], yb)
-        for xi in (x, xh):
-            ya = ops.ln_affine(xi, em[0], em[5], out_dtype=out_dtype)
-            yb = ops.ln_affine(xi[:1000], em[0], em[5], out_dtype=out_dtype)
-            assert torch.equal(ya[:1000], yb)
+    for D in (256, 1024, 1536, 2048):
+        g = torch.Generator(device=DEV).manual_seed(3 + D)
+        qkv = torch.randn(2500, 3 * D, device=DEV, generator=g).bfloat16()
+        w = 1 + 0.1 * torch.randn(2, D, device=DEV, generator=g)
+        cs = torch.randn(2500, 128, device=DEV, generator=g)
+        a, b = qkv.clone(), qkv[:500].clone()
+        ops.rmsnorm_rope_segs_(a, w, 2, cs, 128)         # 5000 items: staged
+        ops.rmsnorm_rope_segs_(b, w, 2, cs[:500], 128)   # 1000 items: register form
+        assert torch.equal(a[:500], b), D
+        x = torch.randn(2500, D, device=DEV, generator=g) * 2 + 0.3
+        em = torch.randn(6, D, device=DEV, generator=g) * 0.2
+        ya = ops.ln_modulate(x, em, 4, 3)
+        yb = ops.ln_modulate(x[:1000], em, 4, 3)
+        assert torch.equal(ya[:1000], yb), D
+        xh = x.bfloat16()
+        for out_dtype in (torch.bfloat16, torch.float32):
+            ya = ops.ln_modulate(xh, em, 1, 0, round_ln_to_bf16=True, out_dtype=out_dtype)
+            yb = ops.ln_modulate(xh[:1000], em, 1, 0, round_ln_to_bf16=True, out_dtype=out_dtype)
+            assert ya.dtype == out_dtype and torch.equal(ya[:1000], yb), (D, out_dtype)
+            for xi in (x, xh):
+                ya = ops.ln_affine(xi, em[0], em[5], out_dtype=out_dtype)
+                yb = ops.ln_affine(xi[:1000], em[0], em[5], out_dtype=out_dtype)
+                assert torch.equal(ya[:1000], yb), (D, out_dtype, xi.dtype)
 
 
 # ------------------------------------------------------------------------------------------- wgmma attention
