@@ -407,6 +407,27 @@ int32_t mc_head_unpatchify_step(const void* x, int32_t x_dtype, const float* r_o
                                 const void* prepared, int64_t prepared_bytes, int32_t flags, const float* cond, const float* x_latent,
                                 float guide_scale, float coef_x, float coef_v, void* stream);
 
+/* Open-Sora 1.2's final layer in one pass (csrc/opensora_head.cu): T2IFinalLayer (videosys/models/transformers/
+ * open_sora_transformer_3d.py:50-86) and `unpatchify` (:625-647), replacing OpenSoraEngine.head's mc_ln_modulate (mode 2) per
+ * sample + mc_gemm_bf16 (MC_EPI_BIAS_BF16, N = 32) + the permute / crop / `.float()` copy, and on a cache hit the mc_cache_hit_add
+ * in front of them (eval/magcache/experiments/opensora.py:344 `x = ori_x + residual`). Per row of x bf16 [B*T*H*W, cols] (sample
+ * b = row / (T*H*W)):
+ *   x   = res_or_null ? bf16(x + res) : x                           (res bf16, same shape; the sum is never written)
+ *   h   = bf16(bf16(bf16(LN(x)) * bf16(1 + scale_b)) + shift_b)     (mc_ln_modulate mode 2, eps; mod fp32 [B, 2, cols] = shift | scale)
+ *   o_j = bf16(sum_k h_k w_jk + bias_j), j < 32                     (the wgmma instruction and K order of mc_gemm_bf16: same bits)
+ *   pred[b, c, t, 2h+p, 2w+q] = o_{(2p+q)*8 + c}, cropped to Hx x Wx (Hx in {2H-1, 2H}, likewise Wx)
+ * Plain mode (z_or_null == NULL): out fp32 [B, 8, T, Hx, Wx] = pred, bit-equal to the op chain.
+ * Step mode (z_or_null != NULL, B even): samples [0, B/2) are the conditional and [B/2, B) the unconditional halves of the CFG
+ * batch; the tail of RFLOW.sample (videosys/schedulers/scheduling_rflow_open_sora.py:244-251) over the 4 velocity channels
+ *   v   = u + g * (c - u),  c = pred[b, ch], u = pred[b + B/2, ch], ch < 4   (`output.chunk(2, dim=1)[0]`, `pred.chunk(2, dim=0)`)
+ *   out[b, ch] = z[b, ch] + v * dt[b]                               (z, out fp32 [B/2, 4, T, Hx, Wx], dt fp32 [B/2] on the device)
+ * each operation rounded on its own in that order (no FMA contraction); out may alias z; pred itself is never written.
+ * w: final_layer.linear.weight bf16 [32, cols]; bias fp32 [32] (bf16 values). cols % 8 == 0, cols <= 1152; C_out must be 8.
+ * x / res / w / mod 16-byte aligned. No workspace. */
+int32_t mc_opensora_head(const void* x, const void* res_or_null, int32_t B, int32_t T, int32_t H, int32_t W, int32_t cols,
+                         const float* mod, const void* w, const float* bias, int32_t C_out, float eps, int32_t Hx, int32_t Wx,
+                         const float* z_or_null, const float* dt, float guidance_scale, float* out, void* stream);
+
 /* bf16 transpose dst[c, r] = src[r, c]. */
 int32_t mc_transpose_bf16(const void* src, int64_t lds, int32_t rows, int32_t cols, void* dst, int64_t ldd, void* stream);
 

@@ -16,7 +16,7 @@ MC_F32, MC_BF16 = 0, 1
 MC_CMP_LT, MC_CMP_LE = 0, 1
 MC_RETAIN_FLOOR, MC_RETAIN_HALF_UP, MC_RETAIN_CEIL, MC_RETAIN_WAN22_T2V, MC_RETAIN_WAN22_I2V, MC_RETAIN_EXPLICIT = 0, 1, 2, 3, 4, 5
 MC_CTRL_SIGNED_ERR, MC_CTRL_RESET_AT_ZERO, MC_CTRL_RATIO_VETO, MC_CTRL_WRAP_KEEPS_ACC = 1, 2, 4, 8
-ABI_VERSION = 6
+ABI_VERSION = 7
 MC_EPI_BIAS_BF16, MC_EPI_BIAS_GELU_BF16, MC_EPI_BIAS_GATE_RESID, MC_EPI_ROWBIAS_BF16, MC_EPI_BIAS_F32, MC_EPI_BIAS_GELU_ERF_BF16 = 0, 1, 2, 3, 4, 5
 MC_EPI_BIAS_GATE_RESID_BF16, MC_EPI_BIAS_SILU_BF16 = 6, 7
 
@@ -131,6 +131,8 @@ SIGNATURES = {
                               POINTER(c_void_p), c_int32, c_void_p, c_int64, c_int32, c_void_p],
     "mc_head_unpatchify_step": [c_void_p, c_int32, c_void_p, c_int64, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32, c_float,
                                 POINTER(c_void_p), c_int32, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_float, c_float, c_float, c_void_p],
+    "mc_opensora_head": [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_float,
+                         c_int32, c_int32, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
     "mc_transpose_bf16": [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p],
     "mc_time_sinusoid": [c_void_p, c_int32, c_int32, c_void_p, c_void_p],
     "mc_cast": [c_void_p, c_int32, c_void_p, c_int32, c_int64, c_void_p],

@@ -140,7 +140,7 @@ static void advance(const mc_ctrl_config* c, mc_ctrl_state* st) {
 extern "C" {
 
 const char* mc_last_error(void) { return mc::g_err; }
-int32_t mc_abi_version(void) { return 6; }
+int32_t mc_abi_version(void) { return 7; }
 
 int32_t mc_nearest_interp(const double* src, int32_t L, double* dst, int32_t T) {
   MC_CHECK_ARG(src && dst, "mc_nearest_interp: null pointer");

@@ -7,6 +7,7 @@
 #include "common.cuh"
 #include "ptx.cuh"
 #include "ring.cuh"
+#include "rowwise.cuh"
 
 namespace mc {
 
@@ -36,39 +37,9 @@ __device__ __forceinline__ void load_row_group(const void* x, int dtype_bf16, in
     ptx::ld_nc_v8_f32(static_cast<const float*>(x) + off, f);
   }
 }
-__device__ __forceinline__ void load_param8(const float* p, float (&f)[8]) {  // per-column parameters: L1-resident, reused by every row
-  const float4 a = __ldg(reinterpret_cast<const float4*>(p)), b = __ldg(reinterpret_cast<const float4*>(p) + 1);
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
-}
 
-// ---- per-row arithmetic: every launch form below calls these, so all forms give the same bits -------------------------------
-// LayerNorm statistics of a row held in registers. Group i of this lane is column group lane + i * lanes; groups at or past
-// `groups` are left out. `reduce` sums over the lanes of the row. Two passes: the mean, then the variance from the squared
-// deviations. Returns rsqrt(var + eps) and sets `mean`.
-template <int G, typename Reduce>
-__device__ __forceinline__ float ln_rstd(const float (&v)[G][8], int lane, int lanes, int groups, float inv_n, float eps, Reduce reduce,
-                                         float& mean) {
-  float s = 0.f;
-#pragma unroll
-  for (int i = 0; i < G; ++i)
-    if (lane + i * lanes < groups) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s += v[i][j];
-    }
-  mean = reduce(s) * inv_n;
-  float q = 0.f;
-#pragma unroll
-  for (int i = 0; i < G; ++i)
-    if (lane + i * lanes < groups) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float d = v[i][j] - mean;
-        q = fmaf(d, d, q);
-      }
-    }
-  return rsqrtf(reduce(q) * inv_n + eps);
-}
-
+// ---- per-row arithmetic: every launch form below calls these (and ln_rstd / t2i_modulate8 of rowwise.cuh), so all forms give
+// the same bits -------------------------------------------------------------------------------------------------------------
 // Output of modes 0 / 1 for 8 elements of a row: y = LN(x) * (1 + a) + b (mode 0) or LN(x) * a + b (mode 1), a and b the
 // per-column parameters at pa / pb, the LN value first rounded to bf16 when round_ln; stored at out + off as bf16 or fp32.
 __device__ __forceinline__ void ln_modulate_store8(const float (&v)[8], float mean, float rstd, const float* pa, const float* pb, int mode,
@@ -97,10 +68,6 @@ __device__ __forceinline__ void rms_weight8(const float (&x)[8], float r, const 
 #pragma unroll
   for (int j = 0; j < 8; ++j) o[j] = round_bf16(x[j] * r) * wv[j];
 }
-
-struct WarpReduce {  // the `reduce` of the warp-per-row forms
-  __device__ __forceinline__ float operator()(float v) const { return warp_sum(v); }
-};
 
 // ---- K7: LayerNorm (no affine) + modulation / affine, optional bf16 rounding of the LN output -----------------
 //   mode 0: y = LN(x) * (1 + p0[scale_idx]) + p0[shift_idx]   with p0 = e = modulation + e0, fp32 [k, cols]
@@ -173,14 +140,8 @@ __global__ void __launch_bounds__(256, (kRelL1 && G < 8) ? 2 : 0) ln_t2i_modulat
     for (int i = 0; i < G; ++i) {
       const int g = lane + i * 32;
       if (g < groups) {
-        float a[8], b[8], o[8];
-        load_param8(sc + g * 8, a);
-        load_param8(sh + g * 8, b);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float y = round_bf16((v[i][j] - mean) * rstd);
-          o[j] = round_bf16(__fadd_rn(round_bf16(__fmul_rn(y, round_bf16(__fadd_rn(1.0f, a[j])))), b[j]));
-        }
+        float o[8];
+        t2i_modulate8(v[i], mean, rstd, sc + g * 8, sh + g * 8, o);
         ptx::st_na_v4(out + row * cols + g * 8, pack_bf16x8(o));
         if constexpr (kRelL1) {
           float p[8];

@@ -121,6 +121,7 @@ class OpenSoraEngine:
         self.w, self.device = weights, weights.device
         self._shape = None
         self.res_valid = False
+        self._step = None  # (z, guidance_scale, dt, out) armed by `arm_step` for the next forward
 
     # ------------------------------------------------------------------------------------------ buffers
     def _alloc(self, B, T, H, W):
@@ -285,18 +286,40 @@ class OpenSoraEngine:
         Tx, Hx, Wx = self.crop
         return o[:, :, :Tx, :Hx, :Wx].float()
 
+    def arm_step(self, z, guidance_scale, dt, out):
+        """Fold the tail of the sampler's step (scheduling_rflow_open_sora.py:244-251: velocity channels, cond / uncond split, CFG
+        combine, `z + v_pred * dt`) into the final layer of the NEXT forward, which then returns `out` = the updated latent fp32
+        [B/2, 4, Tx, Hx, Wx] instead of the prediction (`mc_opensora_head` step mode). z: the latent of this step, fp32 of that
+        shape; dt: fp32 [B/2] on the device; `out` may be `z`. One-shot; bit-equal to the plain forward followed by the reference's
+        statements."""
+        if self.w.out_channels != 8:
+            raise NotImplementedError("magcache_b200: the fused sampler step is built for 8 output channels (pred_sigma)")
+        self._step = (z, float(guidance_scale), dt, out)
+
+    def _final(self, x, hit):
+        """The final layer on `x` (None on a hit: x0 + cached residual): `head`, or the armed step in one `mc_opensora_head` pass."""
+        step, self._step = self._step, None
+        if step is None:
+            return self.head(ops.cache_hit_add(self.x0, self.res, out=self.hit) if hit else x)
+        z, g, dt, out = step
+        return ops.opensora_head(self.x0 if hit else x, self.finf.view(self.B, 2, self.w.dim), self.w.fin_w, self.w.fin_b,
+                                 (self.T, self.H, self.W), self.crop, res=self.res if hit else None, step=(z, g, dt), out=out,
+                                 tag="os_head_step")
+
     def forward(self, kind):
         """prologue -> {hit: x0 + cached residual | miss: blocks, residual = x - x0} -> final layer (opensora.py:309-367)."""
-        self.prologue(kind)
-        if kind == "hit":
-            if not self.res_valid:
-                raise TypeError("magcache_b200: cache hit with an empty residual cache")
-            x = ops.cache_hit_add(self.x0, self.res, out=self.hit)
-        else:
+        try:
+            self.prologue(kind)
+            if kind == "hit":
+                if not self.res_valid:
+                    raise TypeError("magcache_b200: cache hit with an empty residual cache")
+                return self._final(None, True)
             x = self.run_blocks()
             ops.residual_sub(x, self.x0, out=self.res)
             self.res_valid = True
-        return self.head(x)
+            return self._final(x, False)
+        finally:
+            self._step = None
 
     # ------------------------------------------------------------------------------------------ TeaCache (opensora.py:34-227)
     def _tea_alloc(self):
@@ -340,21 +363,26 @@ class OpenSoraEngine:
         """After `prologue("hit")` and `modulated_input`: hit `x += previous_residual` (bf16, :114) | miss: the caption MLP, the block
         stack with block 0's first LN-modulate taken from the decision input (the same tensor), `previous_residual = x - origin_x`
         (:156) -> final layer."""
-        if not calc:
-            if not self.res_valid:
-                raise TypeError("magcache_b200: TeaCache hit with no previous_residual")
-            x = ops.cache_hit_add(self.x0, self.res, out=self.hit)
-        else:
+        try:
+            if not calc:
+                if not self.res_valid:
+                    raise TypeError("magcache_b200: TeaCache hit with no previous_residual")
+                return self._final(None, True)
             self.caption()
             x = self.run_blocks(self.mi[self.mi_prev])
             ops.residual_sub(x, self.x0, out=self.res)
             self.res_valid = True
-        return self.head(x)
+            return self._final(x, False)
+        finally:
+            self._step = None
 
     def forward_plain(self):
         """`enable_teacache = False` (:157-197): the block stack, no residual kept."""
-        self.prologue("miss")
-        return self.head(self.run_blocks())
+        try:
+            self.prologue("miss")
+            return self._final(self.run_blocks(), False)
+        finally:
+            self._step = None
 
 
 def random_opensora_weights(dev, hidden_size=1152, depth=28, num_heads=16, caption_channels=4096, model_max_length=300, seed=0):

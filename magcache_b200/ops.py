@@ -335,6 +335,42 @@ def ln_t2i_modulate(x, em, scale_idx, shift_idx, eps=1e-6, out=None, tag=None):
     return out
 
 
+def opensora_head(x, mod, w, bias, grid, crop, res=None, step=None, out=None, eps=1e-6, tag=None):
+    """Open-Sora's final layer + unpatchify in one pass (`mc_opensora_head`): x bf16 [B*T*H*W, D] (x0 with `res` bf16 on a cache hit,
+    the sum never written), mod fp32 [B, 2, D] (shift | scale per sample), w bf16 [32, D], bias fp32 [32], grid (T, H, W), crop
+    (Tx, Hx, Wx). Returns fp32 [B, 8, Tx, Hx, Wx], bit-equal to OpenSoraEngine.head. With step = (z, guidance_scale, dt) it returns
+    instead `z + (u + g * (c - u)) * dt` over the 4 velocity channels, fp32 [B/2, 4, Tx, Hx, Wx] (c: samples [0, B/2), u: [B/2, B);
+    z fp32 of that shape, dt fp32 [B/2] on the device); `out` may be `z`."""
+    _dev(x, "x")
+    T, H, W = grid
+    Tx, Hx, Wx = crop
+    rows, D = x.shape
+    B = rows // (T * H * W)
+    assert Tx == T and B * T * H * W == rows and x.dtype == torch.bfloat16 and x.is_contiguous()
+    assert res is None or (res.dtype == torch.bfloat16 and res.shape == x.shape and res.is_contiguous())
+    assert mod.dtype == torch.float32 and mod.shape == (B, 2, D) and mod.is_contiguous()
+    assert w.dtype == torch.bfloat16 and w.shape == (32, D) and w.is_contiguous() and bias.dtype == torch.float32 and bias.numel() == 32
+    z = dt = None
+    g = 0.0
+    if step is None:
+        shape = (B, 8, T, Hx, Wx)
+    else:
+        z, g, dt = step
+        shape = (B // 2, 4, T, Hx, Wx)
+        assert B % 2 == 0 and z.dtype == torch.float32 and tuple(z.shape) == shape and z.is_contiguous()
+        _dev(z, "z"), _dev(dt, "dt")
+        assert dt.dtype == torch.float32 and dt.numel() == B // 2 and dt.is_contiguous()
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    assert out.dtype == torch.float32 and tuple(out.shape) == shape and out.is_contiguous()
+    with _Timed(tag, "opensora_head"):
+        check(lib.mc_opensora_head(x.data_ptr(), res.data_ptr() if res is not None else None, B, T, H, W, D, mod.data_ptr(), w.data_ptr(),
+                                   bias.data_ptr(), 8, eps, Hx, Wx, z.data_ptr() if z is not None else None,
+                                   dt.data_ptr() if dt is not None else None, float(g), out.data_ptr(), _stream()))
+    _count()
+    return out
+
+
 REL_L1_MAX_CTAS = 4096  # MC_LN_REL_L1_MAX_CTAS
 
 

@@ -533,11 +533,16 @@ def _opensora_unsupported(self, x_mask, kw):
         raise NotImplementedError("magcache_b200: Open-Sora with skip_y_embedder is not supported")
 
 
+def opensora_engine(self, device):
+    """The Open-Sora engine cached on the module, built on `device` at first use."""
+    return _cached_engine(self, "_mc_opensora_engine", lambda **skw: OpenSoraEngine(OpenSoraWeights.from_module(self, device), **skw))
+
+
 def _opensora_stage(self, x, timestep, y, mask, x_mask, fps, height, width, kw):
     _opensora_unsupported(self, x_mask, kw)
     if not x.is_cuda:
         raise RuntimeError("magcache_b200: x must be a CUDA tensor (no CPU path)")
-    eng = _cached_engine(self, "_mc_opensora_engine", lambda **skw: OpenSoraEngine(OpenSoraWeights.from_module(self, x.device), **skw))
+    eng = opensora_engine(self, x.device)
     eng.stage_inputs(x, timestep, y, mask, fps, height, width)
     return eng
 

@@ -73,6 +73,97 @@ class FlowEulerSampler:
         return cfg_denoise_step(model, x, t, context, context_null, seq_len, guide_scale, coef_v=d, **kw)
 
 
+def timestep_transform(t, model_kwargs, base_resolution=512 * 512, base_num_frames=1, scale=1.0, num_timesteps=1):
+    """Open-Sora's resolution- and length-dependent timestep shift (scheduling_rflow_open_sora.py:47-70), the same torch statements."""
+    t = t / num_timesteps
+    resolution = model_kwargs["height"] * model_kwargs["width"]
+    ratio_space = (resolution / base_resolution).sqrt()
+    if model_kwargs["num_frames"][0] == 1:
+        num_frames = torch.ones_like(model_kwargs["num_frames"])
+    else:
+        num_frames = model_kwargs["num_frames"] // 17 * 5  # the VAE's temporal reduction
+    ratio_time = (num_frames / base_num_frames).sqrt()
+    ratio = ratio_space * ratio_time * scale
+    new_t = ratio * t / (1 + (ratio - 1) * t)
+    return new_t * num_timesteps
+
+
+class OpenSoraRFlowSampler:
+    """`RFLOW.sample` of Open-Sora 1.2 (videosys/schedulers/scheduling_rflow_open_sora.py:164-256) with the same constructor and
+    `sample` signature, so it can stand in for the pipeline's `scheduler`. The timestep schedule, `all_timesteps` and `dt` are the
+    reference's statements, evaluated in torch on the host. Each step is one CFG forward of the doubled batch; when `model` carries
+    an installed Open-Sora forward (`init_magcache_opensora` / `init_teacache_opensora`), the step's tail — velocity channels,
+    cond / uncond split, `uncond + g * (cond - uncond)`, `z + v_pred * dt` — runs inside that forward's final layer
+    (`OpenSoraEngine.arm_step`, `mc_opensora_head`), so the prediction is never written. Any other model runs the reference's torch
+    statements after its forward. Both give the reference's bits."""
+
+    def __init__(self, num_sampling_steps=30, cfg_scale=7.0, num_timesteps=1000, use_timestep_transform=True, use_discrete_timesteps=False):
+        self.num_sampling_steps = num_sampling_steps
+        self.num_timesteps = num_timesteps
+        self.cfg_scale = cfg_scale
+        self.use_discrete_timesteps = use_discrete_timesteps
+        self.use_timestep_transform = use_timestep_transform
+
+    def timesteps(self, batch, model_args):
+        """The per-step timestep tensors [batch] on the host (:208-213)."""
+        timesteps = [(1.0 - i / self.num_sampling_steps) * self.num_timesteps for i in range(self.num_sampling_steps)]
+        if self.use_discrete_timesteps:
+            timesteps = [int(round(t)) for t in timesteps]
+        timesteps = [torch.tensor([t] * batch) for t in timesteps]
+        if self.use_timestep_transform:
+            host_args = {k: model_args[k].cpu() for k in ("height", "width", "num_frames")}
+            timesteps = [timestep_transform(t, host_args, num_timesteps=self.num_timesteps) for t in timesteps]
+        return timesteps
+
+    def dt(self, timesteps, i):
+        """`dt` of step i (:249-250)."""
+        dt = timesteps[i] - timesteps[i + 1] if i < len(timesteps) - 1 else timesteps[i]
+        return dt / self.num_timesteps
+
+    def sample(self, model, z, model_args, y_null, device, mask=None, guidance_scale=None, progress=True, verbose=False):
+        from .patch import magcache_opensora_forward, opensora_engine, teacache_opensora_forward
+        if mask is not None:
+            raise NotImplementedError("magcache_b200: Open-Sora sampling with a mask (image / video conditioning with x_mask) is not supported")
+        if guidance_scale is None:
+            guidance_scale = self.cfg_scale
+        model_args["y"] = torch.cat([model_args["y"], y_null], 0)
+        host_ts = self.timesteps(z.shape[0], model_args)
+        timesteps = [t.to(device) for t in host_ts]
+        dtype = model.x_embedder.proj.weight.dtype
+        # `int(t.to(dtype).item())` (:222) of the first entry: every entry is the same, and the reference's `.item()` of the whole
+        # [B] tensor raises for two or more prompts
+        all_timesteps = [int(t[0].to(dtype).item()) for t in host_ts]
+        eng = None
+        if getattr(type(model), "forward", None) in (magcache_opensora_forward, teacache_opensora_forward):
+            if model.__dict__.get("_mc_shard_kw", {}).get("shard_world", 1) > 1:
+                raise NotImplementedError("magcache_b200: the Open-Sora sampler has no token-sharded path")
+            eng = opensora_engine(model, torch.device(device))
+            z = z.to(device=device, dtype=torch.float32, copy=True)  # the sampler's own latent, updated in place (bf16 -> fp32 is exact)
+        steps = list(enumerate(timesteps))
+        if progress and (not torch.distributed.is_initialized() or torch.distributed.get_rank() == 0):
+            from tqdm import tqdm
+            steps = tqdm(steps)
+        for i, t in steps:
+            z_in = torch.cat([z, z], 0)
+            t = torch.cat([t, t], 0)
+            dt = self.dt(host_ts, i).to(device)
+            if eng is not None:
+                if dt.dtype != torch.float32:
+                    raise NotImplementedError(f"magcache_b200: the fused Open-Sora step takes an fp32 dt (model_args gave {dt.dtype})")
+                eng.arm_step(z, guidance_scale, dt, z)
+                try:
+                    z = model(z_in, t, all_timesteps, **model_args)
+                finally:
+                    eng._step = None
+                continue
+            output = model(z_in, t, all_timesteps, **model_args)
+            pred = output.chunk(2, dim=1)[0]
+            pred_cond, pred_uncond = pred.chunk(2, dim=0)
+            v_pred = pred_uncond + guidance_scale * (pred_cond - pred_uncond)
+            z = z + v_pred * dt[:, None, None, None, None]
+        return z
+
+
 class FlowUniPCSampler:
     """UniPC (bh2, x0-prediction, order 2, lower order on the first and last step, corrector after the first step) on the
     flow parameterisation alpha = 1 - sigma. Two launches per step: [corrector + x0-prediction] and [predictor]."""
