@@ -334,15 +334,19 @@ def test_shape_table_matches_the_engines():
 
 
 # ------------------------------------------------------------------------------------------- (a) one-layer forwards
-def _rule(what, out, ref, exact):
+def _rule(what, out, ref, exact, verbose=True):
+    """DESIGN §5's rule; returns the larger of its two errors as a fraction of its bound."""
     e_ref, e_vs, e_ours = rel_l2(ref, exact), rel_l2(out, ref), rel_l2(out, exact)
-    print(f"  {what}: ours vs fp64 {e_ours:.3e} | oracle(bf16) vs fp64 {e_ref:.3e} | ours vs oracle {e_vs:.3e}")
+    if verbose:
+        print(f"  {what}: ours vs fp64 {e_ours:.3e} | oracle(bf16) vs fp64 {e_ref:.3e} | ours vs oracle {e_vs:.3e}")
     assert e_vs <= 2.0 * e_ref + 1e-3 and e_ours <= 1.5 * e_ref + 1e-3, (what, e_ours, e_ref, e_vs)
+    return max(e_vs / (2.0 * e_ref + 1e-3), e_ours / (1.5 * e_ref + 1e-3))
 
 
-def _forward_loop(name, calls, ours, ref_m, m64, exact_ctx, res_attr, attrs):
+def _forward_loop(name, calls, ours, ref_m, m64, exact_ctx, res_attr, attrs, check=None):
     """Per call: our forward, the bf16 oracle, the fp64 oracle (each result moved to the host at once), then DESIGN §5's rule
-    on the output and on the residual cache, and the controller attributes bit-equal. Returns the oracle's skip decisions."""
+    on the output and on the residual cache, and the controller attributes bit-equal; `check(i, out, ref, ex, r_ours, r_ref,
+    r_ex)`, when given, holds parts of the same host tensors to more rules. Returns the oracle's skip decisions."""
     skips = []
     for i, (args_ours, args_ref, args_64) in enumerate(calls):
         with torch.no_grad():
@@ -360,6 +364,8 @@ def _forward_loop(name, calls, ours, ref_m, m64, exact_ctx, res_attr, attrs):
         assert out.shape == ref.shape == ex.shape
         _rule("output", out, ref, ex)
         _rule("residual cache", r_ours, r_ref, r_ex)
+        if check is not None:
+            check(i, out, ref, ex, r_ours, r_ref, r_ex)
         for a in attrs:
             vals = [np.asarray(getattr(m, a), dtype=np.float64).tolist() for m in (ours, ref_m, m64)]
             assert vals[0] == vals[1] == vals[2], (i, a, vals)
