@@ -348,6 +348,22 @@ int32_t mc_p2p_bump(uint32_t* epoch, uint32_t* own_flag_or_null, void* stream);
 int32_t mc_p2p_push(const void* src, void* const* dst_ptrs, void* const* flag_ptrs, int32_t n_dst, int64_t bytes, const uint32_t* epoch,
                     void* stream);
 int32_t mc_p2p_wait(const uint32_t* flags, int32_t n, const uint32_t* epoch, void* stream);
+/* mc_p2p_push2d: the 2-D form of mc_p2p_push, for Open-Sora's sequence-parallel layout switch. It replaces the `all_to_all_with_pad`
+ * of STDiT3Block.dynamic_switch (videosys/models/transformers/open_sora_transformer_3d.py:275-296, videosys/core/comm.py:297-367)
+ * and the `gather_sequence` in front of the final layer (eval/magcache/experiments/opensora.py:356-361). On `stream`: every copy i,
+ * cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, height) in bytes (any of them may be local or in a peer's window), in list
+ * order; then *epoch (4 bytes) to every flag_ptrs[j]: a peer that observes its flag observes every block. Copies with width or
+ * height 0 are skipped. All arguments are checked before anything is issued. */
+typedef struct mc_copy2d {
+  void* dst;
+  int64_t dpitch;
+  const void* src;
+  int64_t spitch;
+  int64_t width;
+  int64_t height;
+} mc_copy2d;
+int32_t mc_p2p_push2d(const mc_copy2d* copies, int32_t n_copies, void* const* flag_ptrs, int32_t n_flags, const uint32_t* epoch,
+                      void* stream);
 
 /* ---- the collective formulation of the same exchange (SURVEY §8b `mc_nccl_init` / `mc_allgather_kv`; csrc/nccl_gather.cu) ---------
  * `dist.all_gather(tensor_list, input_)` + `torch.cat` of videosys/core/comm.py:272-292 as ONE ncclAllGather on the caller's
@@ -427,6 +443,14 @@ int32_t mc_head_unpatchify_step(const void* x, int32_t x_dtype, const float* r_o
 int32_t mc_opensora_head(const void* x, const void* res_or_null, int32_t B, int32_t T, int32_t H, int32_t W, int32_t cols,
                          const float* mod, const void* w, const float* bias, int32_t C_out, float eps, int32_t Hx, int32_t Wx,
                          const float* z_or_null, const float* dt, float guidance_scale, float* out, void* stream);
+/* mc_opensora_head_frames: mc_opensora_head on one rank's frames of a sequence-parallel run. It replaces the `gather_sequence` of x
+ * in front of the final layer (eval/magcache/experiments/opensora.py:356-361) with a final layer on the rank's own frames. x (and
+ * res) hold T frames of every sample; out and z are tensors of T_out >= T frames, passed pre-offset to the rank's first frame t0
+ * (out + t0 * Hx * Wx, z + t0 * Hx * Wx), so the launch writes frames [t0, t0 + T) of every (sample, channel) and reads the same
+ * frames of z. Every written value has the bits mc_opensora_head writes for that frame of the full tensors. */
+int32_t mc_opensora_head_frames(const void* x, const void* res_or_null, int32_t B, int32_t T, int32_t H, int32_t W, int32_t cols,
+                                const float* mod, const void* w, const float* bias, int32_t C_out, float eps, int32_t Hx, int32_t Wx,
+                                int32_t T_out, const float* z_or_null, const float* dt, float guidance_scale, float* out, void* stream);
 
 /* bf16 transpose dst[c, r] = src[r, c]. */
 int32_t mc_transpose_bf16(const void* src, int64_t lds, int32_t rows, int32_t cols, void* dst, int64_t ldd, void* stream);

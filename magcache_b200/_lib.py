@@ -62,6 +62,10 @@ class DitWeights(Structure):
     _fields_ = [(n, c_void_p) for n in DIT_TOP_FIELDS] + [("blocks", POINTER(DitBlock))]
 
 
+class Copy2D(Structure):
+    _fields_ = [("dst", c_void_p), ("dpitch", c_int64), ("src", c_void_p), ("spitch", c_int64), ("width", c_int64), ("height", c_int64)]
+
+
 class CtrlState(Structure):
     _fields_ = [("cnt", c_int32), ("accumulated_steps", c_int32 * 2), ("pad", c_int32), ("accumulated_ratio", c_double * 2),
                 ("accumulated_err", c_double * 2)]
@@ -122,6 +126,7 @@ SIGNATURES = {
     "mc_p2p_bump": [c_void_p, c_void_p, c_void_p],
     "mc_p2p_push": [c_void_p, POINTER(c_void_p), POINTER(c_void_p), c_int32, c_int64, c_void_p, c_void_p],
     "mc_p2p_wait": [c_void_p, c_int32, c_void_p, c_void_p],
+    "mc_p2p_push2d": [POINTER(Copy2D), c_int32, POINTER(c_void_p), c_int32, c_void_p, c_void_p],
     "mc_linear_f32_small": [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p],
     "mc_head_workspace_bytes": [c_int32, POINTER(c_int64)],
     "mc_head_unpatchify": [c_void_p, c_int32, c_void_p, c_int64, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,
@@ -133,6 +138,8 @@ SIGNATURES = {
                                 POINTER(c_void_p), c_int32, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_float, c_float, c_float, c_void_p],
     "mc_opensora_head": [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_float,
                          c_int32, c_int32, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
+    "mc_opensora_head_frames": [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32,
+                                c_float, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_float, c_void_p, c_void_p],
     "mc_transpose_bf16": [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_int64, c_void_p],
     "mc_time_sinusoid": [c_void_p, c_int32, c_int32, c_void_p, c_void_p],
     "mc_cast": [c_void_p, c_int32, c_void_p, c_int32, c_int64, c_void_p],

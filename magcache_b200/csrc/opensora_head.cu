@@ -57,11 +57,12 @@ struct OsHeadParams {
   const float* mod;          // [B, 2, cols] shift | scale per sample, bf16 values
   int64_t N;                 // rows per sample: T H W
   int B, cols, T, H, W, Hx, Wx;
+  int T_out;                 // frames of the output (and z) tensor: T, or more when `out` / `z` point at a frame window of it
   float eps;
   const float* z;            // step mode: [B/2, C/2, T, Hx, Wx]; nullptr: plain mode
   const float* dt;           // step mode: [B/2]
   float g;
-  float* out;                // plain: [B, C, T, Hx, Wx]; step: [B/2, C/2, T, Hx, Wx] (may alias z)
+  float* out;                // plain: [B, C, T_out, Hx, Wx]; step: [B/2, C/2, T_out, Hx, Wx] (may alias z)
 };
 
 template <bool HIT>
@@ -183,11 +184,11 @@ __global__ void __launch_bounds__(osh::kThreads, 1) opensora_head_kernel(const O
             const int c = 2 * (lane & 3) + e, j = 8 * i + c;
             const float y = round_bf16(acc[4 * i + 2 * h + e] + __ldg(p.bias + j));
             if (!step) {
-              if (in) p.out[((b * kC + c) * p.T + t) * plane + static_cast<int64_t>(yy) * p.Wx + xx] = y;
+              if (in) p.out[((b * kC + c) * p.T_out + t) * plane + static_cast<int64_t>(yy) * p.Wx + xx] = y;
             } else if (pass == 0) {
               keep[4 * i + 2 * h + e] = y;
             } else if (in && c < kC / 2) {
-              const int64_t o = ((b * (kC / 2) + c) * p.T + t) * plane + static_cast<int64_t>(yy) * p.Wx + xx;
+              const int64_t o = ((b * (kC / 2) + c) * p.T_out + t) * plane + static_cast<int64_t>(yy) * p.Wx + xx;
               const float vel = __fadd_rn(y, __fmul_rn(p.g, __fsub_rn(keep[4 * i + 2 * h + e], y)));  // uncond + g * (cond - uncond)
               p.out[o] = __fadd_rn(p.z[o], __fmul_rn(vel, __ldg(p.dt + b)));                         // z + v_pred * dt
             }
@@ -200,21 +201,23 @@ __global__ void __launch_bounds__(osh::kThreads, 1) opensora_head_kernel(const O
 
 }  // namespace mc
 
-extern "C" int32_t mc_opensora_head(const void* x, const void* res_or_null, int32_t B, int32_t T, int32_t H, int32_t W, int32_t cols,
-                                    const float* mod, const void* w, const float* bias, int32_t C_out, float eps, int32_t Hx, int32_t Wx,
-                                    const float* z_or_null, const float* dt, float guidance_scale, float* out, void* stream) {
+namespace {
+int32_t opensora_head_launch(const char* fn, const void* x, const void* res_or_null, int32_t B, int32_t T, int32_t H, int32_t W,
+                             int32_t cols, const float* mod, const void* w, const float* bias, int32_t C_out, float eps, int32_t Hx,
+                             int32_t Wx, int32_t T_out, const float* z_or_null, const float* dt, float guidance_scale, float* out,
+                             void* stream) {
   using namespace mc;
-  MC_CHECK_ARG(x && mod && w && bias && out, "mc_opensora_head: null pointer");
-  MC_CHECK_ARG(C_out == osh::kC, "mc_opensora_head: built for patch (1, 2, 2) x 8 output channels (32 features), got C_out=%d", C_out);
-  MC_CHECK_ARG(cols >= 8 && cols % 8 == 0 && cols <= osh::kMaxCols, "mc_opensora_head: cols=%d must be a multiple of 8 in [8, %d]", cols,
+  MC_CHECK_ARG(x && mod && w && bias && out, "%s: null pointer", fn);
+  MC_CHECK_ARG(C_out == osh::kC, "%s: built for patch (1, 2, 2) x 8 output channels (32 features), got C_out=%d", fn, C_out);
+  MC_CHECK_ARG(cols >= 8 && cols % 8 == 0 && cols <= osh::kMaxCols, "%s: cols=%d must be a multiple of 8 in [8, %d]", fn, cols,
                osh::kMaxCols);
-  MC_CHECK_ARG(B >= 1 && T >= 1 && H >= 1 && W >= 1, "mc_opensora_head: bad shape B=%d T=%d H=%d W=%d", B, T, H, W);
+  MC_CHECK_ARG(B >= 1 && T >= 1 && H >= 1 && W >= 1, "%s: bad shape B=%d T=%d H=%d W=%d", fn, B, T, H, W);
+  MC_CHECK_ARG(T_out >= T, "%s: the output holds %d frames, fewer than the %d of x", fn, T_out, T);
   MC_CHECK_ARG(Hx >= 2 * H - 1 && Hx <= 2 * H && Wx >= 2 * W - 1 && Wx <= 2 * W,
-               "mc_opensora_head: crop %d x %d does not match the %d x %d patch grid", Hx, Wx, H, W);
+               "%s: crop %d x %d does not match the %d x %d patch grid", fn, Hx, Wx, H, W);
   MC_CHECK_ARG(aligned16(x) && (res_or_null == nullptr || aligned16(res_or_null)) && aligned16(w) && aligned16(mod),
-               "mc_opensora_head: x / res / w / mod must be 16-byte aligned");
-  MC_CHECK_ARG(z_or_null == nullptr || (B % 2 == 0 && dt != nullptr),
-               "mc_opensora_head: step mode needs an even B (cond | uncond halves) and dt");
+               "%s: x / res / w / mod must be 16-byte aligned", fn);
+  MC_CHECK_ARG(z_or_null == nullptr || (B % 2 == 0 && dt != nullptr), "%s: step mode needs an even B (cond | uncond halves) and dt", fn);
   OsHeadParams p{};
   p.x = static_cast<const __nv_bfloat16*>(x);
   p.res = static_cast<const __nv_bfloat16*>(res_or_null);
@@ -222,6 +225,7 @@ extern "C" int32_t mc_opensora_head(const void* x, const void* res_or_null, int3
   p.bias = bias, p.mod = mod;
   p.N = static_cast<int64_t>(T) * H * W;
   p.B = B, p.cols = cols, p.T = T, p.H = H, p.W = W, p.Hx = Hx, p.Wx = Wx;
+  p.T_out = T_out;
   p.eps = eps;
   p.z = z_or_null, p.dt = dt, p.g = guidance_scale;
   p.out = out;
@@ -239,4 +243,22 @@ extern "C" int32_t mc_opensora_head(const void* x, const void* res_or_null, int3
     opensora_head_kernel<false><<<grid, osh::kThreads, smem, static_cast<cudaStream_t>(stream)>>>(p);
   MC_CHECK_LAUNCH("opensora_head_kernel launch");
   return MC_OK;
+}
+}  // namespace
+
+extern "C" int32_t mc_opensora_head(const void* x, const void* res_or_null, int32_t B, int32_t T, int32_t H, int32_t W, int32_t cols,
+                                    const float* mod, const void* w, const float* bias, int32_t C_out, float eps, int32_t Hx, int32_t Wx,
+                                    const float* z_or_null, const float* dt, float guidance_scale, float* out, void* stream) {
+  return opensora_head_launch("mc_opensora_head", x, res_or_null, B, T, H, W, cols, mod, w, bias, C_out, eps, Hx, Wx, T, z_or_null, dt,
+                              guidance_scale, out, stream);
+}
+
+// The sequence-parallel final layer: x holds one rank's T frames of every sample, out / z point at frame t0 of tensors of T_out
+// frames, so each rank writes its own frame window of the full-size prediction (or updated latent) in place.
+extern "C" int32_t mc_opensora_head_frames(const void* x, const void* res_or_null, int32_t B, int32_t T, int32_t H, int32_t W,
+                                           int32_t cols, const float* mod, const void* w, const float* bias, int32_t C_out, float eps,
+                                           int32_t Hx, int32_t Wx, int32_t T_out, const float* z_or_null, const float* dt,
+                                           float guidance_scale, float* out, void* stream) {
+  return opensora_head_launch("mc_opensora_head_frames", x, res_or_null, B, T, H, W, cols, mod, w, bias, C_out, eps, Hx, Wx, T_out,
+                              z_or_null, dt, guidance_scale, out, stream);
 }

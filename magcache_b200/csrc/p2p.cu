@@ -9,6 +9,8 @@
 //     segment it needs next (ld.acquire.sys in the TMA-issuing warp): the transfer hides behind the math instead of a barrier;
 //   * the head kernel stores its rows straight into every peer's output tensor (mc_head_unpatchify_ex, n_out = world), followed
 //     by a flag per peer and a one-thread wait kernel (mc_p2p_wait).
+//   * Open-Sora's sequence-parallel layout switch (frames <-> positions, videosys/core/comm.py:297-367 `all_to_all_with_pad`) and its
+//     output assembly move strided blocks: mc_p2p_push2d issues one cudaMemcpy2DAsync per (sample, peer) block, then the flags.
 // Flags carry a monotonically increasing epoch kept in device memory (mc_p2p_bump), so that a captured CUDA graph of a whole
 // forward can be replayed: nothing epoch-dependent is baked into a launch.
 #include "common.cuh"
@@ -108,6 +110,36 @@ int32_t mc_p2p_push(const void* src, void* const* dst_ptrs, void* const* flag_pt
     // same stream, after the data: a peer that observes the flag also observes the segment
     cudaError_t e = cudaMemcpyAsync(flag_ptrs[i], epoch, sizeof(uint32_t), cudaMemcpyDefault, s);
     if (e != cudaSuccess) return mc::cuda_fail(e, "mc_p2p_push: flag copy");
+  }
+  return MC_OK;
+}
+
+int32_t mc_p2p_push2d(const mc_copy2d* copies, int32_t n_copies, void* const* flag_ptrs, int32_t n_flags, const uint32_t* epoch,
+                      void* stream) {
+  MC_CHECK_ARG(n_copies >= 0 && n_flags >= 0 && (n_copies == 0 || copies != nullptr) && (n_flags == 0 || (flag_ptrs != nullptr && epoch != nullptr)),
+               "mc_p2p_push2d: bad arguments");
+  // every argument is checked before the first copy is issued: a refused call moves nothing
+  for (int i = 0; i < n_copies; ++i) {
+    const mc_copy2d& c = copies[i];
+    MC_CHECK_ARG(c.width >= 0 && c.height >= 0, "mc_p2p_push2d: copy %d has width %lld, height %lld", i, (long long)c.width, (long long)c.height);
+    if (c.width == 0 || c.height == 0) continue;
+    MC_CHECK_ARG(c.dst != nullptr && c.src != nullptr, "mc_p2p_push2d: copy %d has a null pointer", i);
+    MC_CHECK_ARG(c.dpitch >= c.width && c.spitch >= c.width, "mc_p2p_push2d: copy %d has a pitch below its width (%lld, %lld < %lld)", i,
+                 (long long)c.dpitch, (long long)c.spitch, (long long)c.width);
+  }
+  for (int i = 0; i < n_flags; ++i) MC_CHECK_ARG(flag_ptrs[i] != nullptr, "mc_p2p_push2d: flag %d is null", i);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  for (int i = 0; i < n_copies; ++i) {
+    const mc_copy2d& c = copies[i];
+    if (c.width == 0 || c.height == 0) continue;
+    cudaError_t e = cudaMemcpy2DAsync(c.dst, static_cast<size_t>(c.dpitch), c.src, static_cast<size_t>(c.spitch), static_cast<size_t>(c.width),
+                                      static_cast<size_t>(c.height), cudaMemcpyDefault, s);
+    if (e != cudaSuccess) return mc::cuda_fail(e, "mc_p2p_push2d: data copy");
+  }
+  // same stream, after every block: a peer that observes its flag also observes the blocks
+  for (int i = 0; i < n_flags; ++i) {
+    cudaError_t e = cudaMemcpyAsync(flag_ptrs[i], epoch, sizeof(uint32_t), cudaMemcpyDefault, s);
+    if (e != cudaSuccess) return mc::cuda_fail(e, "mc_p2p_push2d: flag copy");
   }
   return MC_OK;
 }

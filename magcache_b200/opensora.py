@@ -13,12 +13,22 @@ HBM layout (B samples, T frames, S = H*W patches per frame, N = T*S, R = B*N row
   h    [R, D]   LN + t2i_modulate output         qkv [R, 3D] q | k | v, q / k normalised in place  att [R, D]  attention output
   ff   [R, 4D]  MLP hidden                        yk  [L, 2D] cross-attention k | v of the L = sum(y_lens) caption tokens
   mod  [2*depth, B, 6D] per-block `scale_shift_table + t_mlp` (bf16, and an exact fp32 copy for the kernels)
+
+Sequence parallelism (VideoSys DSP, eval/magcache/experiments/opensora.py:284-293, 342-361; `enable_sequence_parallel`): rank r of P
+owns frames [t0, t0 + T_r) (`shard.frame_position_shards`, the `split_sequence` partition without its pad). x / x0 / res / h / att
+then hold those frames of every sample (N = T_r S rows per sample); the spatial blocks and cross-attention run on them unchanged.
+A temporal block switches its modulated input to the position-sharded layout (every frame of positions [s0, s0 + S_r)), runs
+qkv, q / k RMSNorm + RoPE and the attention there, switches the attention output back and runs `proj` with its gated residual on
+the rank's frames (STDiT3Block.dynamic_switch, open_sora_transformer_3d.py:275-296, moves the same D-wide rows). The final layer
+runs on the rank's frames into its window of the full-size output, which the peers then fill in: every rank returns the whole
+prediction (or updated latent). Every row is computed by the launches the one-GPU engine uses for it, so the outputs are the same
+bits.
 """
 import math
 
 import torch
 
-from . import _lib, ops
+from . import _lib, ops, shard
 
 E = _lib
 
@@ -115,10 +125,13 @@ class OpenSoraEngine:
     """One STDiT3 on the sm_90a kernels. Buffers are allocated once per (B, T, H, W) shape; the caption buffer grows with the
     number of valid caption tokens."""
 
-    def __init__(self, weights: OpenSoraWeights, shard_world=1, shard_rank=0, shard_group=None):
+    def __init__(self, weights: OpenSoraWeights, shard_world=1, shard_rank=0, shard_group=None, sp_world=1, sp_rank=0, sp_group=None):
         if shard_world > 1:  # no token-sharded path: every rank would compute the whole video
-            raise NotImplementedError("magcache_b200: Open-Sora token sharding (enable_token_shard with world > 1) is not supported")
+            raise NotImplementedError("magcache_b200: Open-Sora token sharding (enable_token_shard with world > 1) is not supported; "
+                                      "enable_sequence_parallel shards frames and positions instead")
         self.w, self.device = weights, weights.device
+        self.sp = (sp_rank, sp_world, sp_group) if sp_world > 1 else None  # sequence parallelism: (rank, world, group)
+        self.switch = None
         self._shape = None
         self.res_valid = False
         self._step = None  # (z, guidance_scale, dt, out) armed by `arm_step` for the next forward
@@ -129,14 +142,24 @@ class OpenSoraEngine:
             return
         w, dev = self.w, self.device
         D = w.dim
-        S, N = H * W, T * H * W
+        S = H * W
+        self.t0, self.T_loc = 0, T  # this rank's frames (all of them without sequence parallelism)
+        if self.sp is not None:
+            rank, world, group = self.sp
+            frames, positions = shard.frame_position_shards(world, T, S, group)
+            self.t0, self.T_loc, self.S_loc = frames[rank].start, frames[rank].n_local, positions[rank].n_local
+        N = self.T_loc * S  # rows per sample on this rank
         R = B * N
         bf = dict(dtype=torch.bfloat16, device=dev)
-        self.B, self.T, self.H, self.W, self.S, self.N, self.R = B, T, H, W, S, N, R
+        self.B, self.T, self.H, self.W, self.S, self.N = B, T, H, W, S, N
+        self.R = B * T * S  # rows of the whole batch (TeaCache's decision input covers all of them on every rank)
         self.x, self.x0, self.res, self.hit = (torch.empty(R, D, **bf) for _ in range(4))
         self.h, self.att = torch.empty(R, D, **bf), torch.empty(R, D, **bf)
         self.qkv, self.ff = torch.empty(R, 3 * D, **bf), torch.empty(R, 4 * D, **bf)
         self.qc = torch.empty(R, D, **bf)
+        if self.sp is not None:
+            R_pos = B * T * self.S_loc  # position-sharded rows of the temporal attention
+            self.qkv_pos, self.att_pos = torch.empty(R_pos, 3 * D, **bf), torch.empty(R_pos, D, **bf)
         self.mod = torch.empty(2 * w.depth, B, 6 * D, **bf)
         self.mod_t = torch.empty_like(self.mod)
         self.tables_rep = w.tables[:, None, :].expand(2 * w.depth, B, 6 * D).contiguous()
@@ -144,7 +167,7 @@ class OpenSoraEngine:
         self.fin, self.fin_t = torch.empty(B, 2 * D, **bf), torch.empty(B, 2 * D, **bf)
         self.fin_rep = w.fin_table[None].expand(B, 2 * D).contiguous()
         self.finf = torch.empty(B, 2 * D, dtype=torch.float32, device=dev)
-        segs = [(b * N + t * S, S, b * N + t * S, S) for b in range(B) for t in range(T)]  # one spatial segment per frame
+        segs = [(b * N + t * S, S, b * N + t * S, S) for b in range(B) for t in range(self.T_loc)]  # one spatial segment per frame
         self.segs_sp = torch.tensor(segs, dtype=torch.int32, device=dev)
         self.rope = rope_table(T, 72, dev)
         self.s_lat = torch.empty(B, w.in_channels, T, 2 * H, 2 * W, dtype=torch.float32, device=dev)
@@ -153,6 +176,7 @@ class OpenSoraEngine:
         self._y_key = None
         self.res_valid = False
         self._shape = (B, T, H, W)
+        self._crop_key = None
 
     def rows(self, b):
         return slice(b * self.N, (b + 1) * self.N)
@@ -166,6 +190,12 @@ class OpenSoraEngine:
         T, H, W = Tx, -(-Hx // 2), -(-Wx // 2)
         self._alloc(B, T, H, W)
         self.crop = (Tx, Hx, Wx)
+        if self.sp is not None and self._crop_key != (Hx, Wx):  # the output slots are sized by the crop
+            if self.switch is not None:
+                self.switch.close()
+            rank, world, group = self.sp
+            self.switch = shard.make_switch(rank, world, B, T, H * W, w.dim, Hx, Wx, self.device, group)
+            self._crop_key = (Hx, Wx)
         if Hx % 2 or Wx % 2:
             self.s_lat.zero_()  # OpenSoraPatchEmbed3D zero-pads odd H / W
         self.s_lat[:, :, :, :Hx, :Wx].copy_(x.to(torch.bfloat16))  # `x.to(dtype)` (:245), held exactly in fp32
@@ -215,11 +245,7 @@ class OpenSoraEngine:
     def prologue(self, kind):
         """x_embedder + pos_embed into x0, t / fps embedders, t_block, the per-block modulation and, on a miss, the caption MLP."""
         w, B, D = self.w, self.B, self.w.dim
-        x0 = self.x0.view(B, self.T, self.S, D)
-        x0.copy_(self.pos.view(1, 1, self.S, D).expand_as(x0))
-        for b in range(B):  # Conv3d (1,2,2) as a K = 4*C GEMM; `x + pos_emb` in the epilogue (bf16(pos + bf16(acc + bias)))
-            tok = ops.patchify(self.s_lat[b])
-            ops.gemm(tok, w.x_w, w.x_b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=self.x0[self.rows(b)])
+        self._embed(self.x0, self.T_loc, self.t0)
         t = self._time_mlp(self._sinusoid(self.s_t[:B]), w.t_mlp)
         t = ops.cache_hit_add(t, self._time_mlp(self._sinusoid(self.s_t[B:]), w.fps_mlp))  # `t = t + fps` (bf16)
         t_mlp = ops.gemm(ops.silu(t), w.tb_w, w.tb_b, E.MC_EPI_BIAS_BF16)               # t_block
@@ -230,6 +256,17 @@ class OpenSoraEngine:
         ops.cast_into(ops.cache_hit_add(self.fin_rep, self.fin_t, out=self.fin), self.finf)  # final layer `table[None] + t[:, None]`
         if kind == "miss":
             self.caption()
+
+    def _embed(self, x0, T, t0):
+        """x_embedder + pos_embed of frames [t0, t0 + T) of every sample into x0 [B T S, D]."""
+        w, B, D, S = self.w, self.B, self.w.dim, self.S
+        x0v = x0.view(B, T, S, D)
+        x0v.copy_(self.pos.view(1, 1, S, D).expand_as(x0v))
+        for b in range(B):  # Conv3d (1,2,2) as a K = 4*C GEMM; `x + pos_emb` in the epilogue (bf16(pos + bf16(acc + bias)))
+            tok = ops.patchify(self.s_lat[b])
+            if T != self.T:  # the GEMM is row-local: a rank's frames are the same bits as in the whole video
+                tok = tok[t0 * S:(t0 + T) * S]
+            ops.gemm(tok, w.x_w, w.x_b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=x0[b * T * S:(b + 1) * T * S])
 
     def caption(self):
         """The caption MLP (`y_embedder`), which only the block stack reads."""
@@ -246,13 +283,18 @@ class OpenSoraEngine:
             for b in range(B):
                 ops.ln_t2i_modulate(x[self.rows(b)], em[b], 1, 0, out=h[self.rows(b)])
             x_m = h
+        S = self.S
+        if blk["temporal"] and self.sp is not None:  # to every frame of this rank's positions (dynamic_switch, :275-296)
+            x_m, qkv, att, S = self.switch.to_positions(x_m), self.qkv_pos, self.att_pos, self.S_loc
         ops.gemm(x_m, blk["qkv_w"], blk["qkv_b"], E.MC_EPI_BIAS_BF16, out=qkv)
         q, k, v = qkv[:, :D], qkv[:, D:2 * D], qkv[:, 2 * D:]
         rope = self.rope if blk["temporal"] else None
-        ops.rmsnorm_head72_rope_(q, blk["nq"], H, rope, pos_div=self.S, tag="os_qknorm")
-        ops.rmsnorm_head72_rope_(k, blk["nk"], H, rope, pos_div=self.S, tag="os_qknorm")
+        ops.rmsnorm_head72_rope_(q, blk["nq"], H, rope, pos_div=S, tag="os_qknorm")
+        ops.rmsnorm_head72_rope_(k, blk["nk"], H, rope, pos_div=S, tag="os_qknorm")
         if blk["temporal"]:
-            ops.attention_temporal_d72(q, k, v, H, B, self.T, self.S, out=att, tag="os_attn_temporal")
+            ops.attention_temporal_d72(q, k, v, H, B, self.T, S, out=att, tag="os_attn_temporal")
+            if self.sp is not None:  # the attention output back to this rank's frames; `proj` runs there
+                att = self.switch.to_frames(att)
         else:
             ops.attention_varlen_d72(q, k, v, H, self.segs_sp, self.S, out=att, tag="os_attn_spatial")
         for b in range(B):  # `x = x + gate_msa * x_m`
@@ -260,8 +302,8 @@ class OpenSoraEngine:
         # cross-attention (varlen over the caption tokens of each sample), `x = x + x_cross`
         ops.gemm(x, blk["cq_w"], blk["cq_b"], E.MC_EPI_BIAS_BF16, out=self.qc)
         kv = ops.gemm(self.y_emb, blk["ckv_w"], blk["ckv_b"], E.MC_EPI_BIAS_BF16)
-        ops.attention_varlen_d72(self.qc, kv[:, :D], kv[:, D:], H, self.segs_cross, self.N, out=att, tag="os_attn_cross")
-        ops.gemm(att, blk["co_w"], blk["co_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=x)
+        ops.attention_varlen_d72(self.qc, kv[:, :D], kv[:, D:], H, self.segs_cross, self.N, out=self.att, tag="os_attn_cross")
+        ops.gemm(self.att, blk["co_w"], blk["co_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=x)
         # MLP, `x = x + gate_mlp * mlp(t2i_modulate(norm2(x), shift_mlp, scale_mlp))`
         for b in range(B):
             ops.ln_t2i_modulate(x[self.rows(b)], em[b], 4, 3, out=h[self.rows(b)])
@@ -299,12 +341,25 @@ class OpenSoraEngine:
     def _final(self, x, hit):
         """The final layer on `x` (None on a hit: x0 + cached residual): `head`, or the armed step in one `mc_opensora_head` pass."""
         step, self._step = self._step, None
+        if self.sp is not None:
+            return self._final_sp(x, hit, step)
         if step is None:
             return self.head(ops.cache_hit_add(self.x0, self.res, out=self.hit) if hit else x)
         z, g, dt, out = step
         return ops.opensora_head(self.x0 if hit else x, self.finf.view(self.B, 2, self.w.dim), self.w.fin_w, self.w.fin_b,
                                  (self.T, self.H, self.W), self.crop, res=self.res if hit else None, step=(z, g, dt), out=out,
                                  tag="os_head_step")
+
+    def _final_sp(self, x, hit, step):
+        """The final layer on this rank's frames into its window of a full-size output (`mc_opensora_head_frames`), then the peers'
+        windows: every rank returns the whole prediction, or with a step armed the whole updated latent (into the step's `out`)."""
+        _, Hx, Wx = self.crop
+        buf = self.switch.output_buffer(step is not None)
+        z, g, dt, out = step if step is not None else (None, 0.0, None, None)
+        ops.opensora_head_frames(self.x0 if hit else x, self.finf.view(self.B, 2, self.w.dim), self.w.fin_w, self.w.fin_b,
+                                 (self.T_loc, self.H, self.W), (self.T, Hx, Wx), self.t0, buf, res=self.res if hit else None,
+                                 step=(z, g, dt) if step is not None else None, tag="os_head_frames")
+        return self.switch.gather_output(buf, out)
 
     def forward(self, kind):
         """prologue -> {hit: x0 + cached residual | miss: blocks, residual = x - x0} -> final layer (opensora.py:309-367)."""
@@ -327,6 +382,8 @@ class OpenSoraEngine:
             return
         self.mi = torch.empty(2, self.R, self.w.dim, dtype=torch.bfloat16, device=self.device)  # modulated inputs, alternating
         self.mi_prev = None  # index of the buffer holding `previous_modulated_input`, None: there is none
+        if self.sp is not None:  # every frame's x0, for the decision input over all rows
+            self.x0_all = torch.empty(self.R, self.w.dim, dtype=torch.bfloat16, device=self.device)
         self.tea_sums = torch.zeros(2, dtype=torch.float64, device=self.device)
         self.tea_partials = ops.rel_l1_partials(self.device)
         self._tea_shape = self._shape
@@ -347,15 +404,20 @@ class OpenSoraEngine:
         self._tea_alloc()
         k = 0 if self.mi_prev is None else 1 - self.mi_prev
         cur, D = self.mi[k], self.w.dim
+        x0, rows = self.x0, self.rows
+        if self.sp is not None:  # the reference forms it before its split: every rank embeds and modulates all frames
+            self._embed(self.x0_all, self.T, 0)
+            N = self.T * self.S
+            x0, rows = self.x0_all, lambda b: slice(b * N, (b + 1) * N)
         if distance:
             prev = self.mi[self.mi_prev]
             self.tea_sums.zero_()
             for b in range(self.B):
-                ops.ln_t2i_modulate_rel_l1(self.x0[self.rows(b)], self.modf[0, b].view(6, D), 1, 0, prev[self.rows(b)], cur[self.rows(b)],
+                ops.ln_t2i_modulate_rel_l1(x0[rows(b)], self.modf[0, b].view(6, D), 1, 0, prev[rows(b)], cur[rows(b)],
                                            self.tea_partials, self.tea_sums, tag="os_tea_input")
         else:
             for b in range(self.B):
-                ops.ln_t2i_modulate(self.x0[self.rows(b)], self.modf[0, b].view(6, D), 1, 0, out=cur[self.rows(b)], tag="os_tea_input")
+                ops.ln_t2i_modulate(x0[rows(b)], self.modf[0, b].view(6, D), 1, 0, out=cur[rows(b)], tag="os_tea_input")
         self.mi_prev = k
         return self.tea_sums.tolist() if distance else None
 
@@ -369,7 +431,13 @@ class OpenSoraEngine:
                     raise TypeError("magcache_b200: TeaCache hit with no previous_residual")
                 return self._final(None, True)
             self.caption()
-            x = self.run_blocks(self.mi[self.mi_prev])
+            x_m0 = self.mi[self.mi_prev]
+            if self.sp is not None:  # this rank's frames of the decision input
+                N, S = self.T * self.S, self.S
+                for b in range(self.B):
+                    self.h[self.rows(b)].copy_(x_m0[b * N + self.t0 * S:b * N + (self.t0 + self.T_loc) * S])
+                x_m0 = self.h
+            x = self.run_blocks(x_m0)
             ops.residual_sub(x, self.x0, out=self.res)
             self.res_valid = True
             return self._final(x, False)

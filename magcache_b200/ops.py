@@ -371,6 +371,39 @@ def opensora_head(x, mod, w, bias, grid, crop, res=None, step=None, out=None, ep
     return out
 
 
+def opensora_head_frames(x, mod, w, bias, grid, crop, t0, out, res=None, step=None, eps=1e-6, tag=None):
+    """`opensora_head` on frames [t0, t0 + T) of a sequence-parallel run (`mc_opensora_head_frames`): x bf16 [B*T*H*W, D] holds those
+    frames of every sample, grid = (T, H, W) local, crop = (T_out, Hx, Wx) the full tensor. `out` is the full-size fp32 tensor
+    [B, 8, T_out, Hx, Wx] (step mode: [B/2, 4, T_out, Hx, Wx], z of that shape, may alias out): only the window's frames are
+    written (and read of z), bit-equal to the same frames of one `opensora_head` over the whole video."""
+    _dev(x, "x"), _dev(out, "out")
+    T, H, W = grid
+    T_out, Hx, Wx = crop
+    rows, D = x.shape
+    B = rows // (T * H * W)
+    assert 0 <= t0 and t0 + T <= T_out and B * T * H * W == rows and x.dtype == torch.bfloat16 and x.is_contiguous()
+    assert res is None or (res.dtype == torch.bfloat16 and res.shape == x.shape and res.is_contiguous())
+    assert mod.dtype == torch.float32 and mod.shape == (B, 2, D) and mod.is_contiguous()
+    assert w.dtype == torch.bfloat16 and w.shape == (32, D) and w.is_contiguous() and bias.dtype == torch.float32 and bias.numel() == 32
+    z = dt = None
+    g = 0.0
+    shape = (B, 8, T_out, Hx, Wx)
+    if step is not None:
+        z, g, dt = step
+        shape = (B // 2, 4, T_out, Hx, Wx)
+        assert B % 2 == 0 and z.dtype == torch.float32 and tuple(z.shape) == shape and z.is_contiguous()
+        _dev(z, "z"), _dev(dt, "dt")
+        assert dt.dtype == torch.float32 and dt.numel() == B // 2 and dt.is_contiguous()
+    assert out.dtype == torch.float32 and tuple(out.shape) == shape and out.is_contiguous()
+    off = t0 * Hx * Wx * 4
+    with _Timed(tag, "opensora_head"):
+        check(lib.mc_opensora_head_frames(x.data_ptr(), res.data_ptr() if res is not None else None, B, T, H, W, D, mod.data_ptr(),
+                                          w.data_ptr(), bias.data_ptr(), 8, eps, Hx, Wx, T_out, z.data_ptr() + off if z is not None else None,
+                                          dt.data_ptr() if dt is not None else None, float(g), out.data_ptr() + off, _stream()))
+    _count()
+    return out
+
+
 REL_L1_MAX_CTAS = 4096  # MC_LN_REL_L1_MAX_CTAS
 
 

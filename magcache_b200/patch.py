@@ -53,10 +53,29 @@ def enable_token_shard(model, rank, world, group=None):
     """Shard the token axis of `model`'s forwards over `world` ranks of one node (call before the first forward; needs an
     initialised torch.distributed NCCL group). Every rank must then make the same calls with the same inputs; outputs are
     replicated, the residual cache stays sharded. Wan engines shard all tokens; the FLUX / HunyuanVideo engines shard the image tokens and
-    replicate the text tokens. The Open-Sora engine has no sharded path: its forward raises NotImplementedError for world > 1."""
+    replicate the text tokens. The Open-Sora engine has no token-sharded path: its forward raises NotImplementedError for world > 1
+    (`enable_sequence_parallel` shards it by frames and positions instead)."""
     if any(k in model.__dict__ for k in ENGINE_ATTRS):
         raise RuntimeError("enable_token_shard must be called before the first forward")
     object.__setattr__(model, "_mc_shard_kw", dict(shard_world=world, shard_rank=rank, shard_group=group))
+    return model
+
+
+def enable_sequence_parallel(model, rank, world, group=None):
+    """Run `model`'s Open-Sora forwards (`magcache_opensora_forward`, `teacache_opensora_forward`) and `OpenSoraRFlowSampler.sample`
+    with VideoSys's sequence parallelism over `world` ranks of one node: each rank owns a contiguous block of latent frames for the
+    spatial blocks and of positions for the temporal blocks (eval/magcache/experiments/opensora.py:284-293, 342-361). Call before the
+    first forward, after `init_magcache_opensora` / `init_teacache_opensora`, on every rank with an initialised torch.distributed
+    group (`group`, default the world); every rank then makes the same calls with the same inputs (the same latent noise included)
+    and receives the whole output. The residual cache stays sharded: `residual_cache` / `previous_residual` hold this rank's frames.
+    Every output is bit-equal to the one-GPU engine's. world == 1 is the unsharded engine."""
+    if getattr(type(model), "forward", None) not in (magcache_opensora_forward, teacache_opensora_forward):
+        raise RuntimeError("enable_sequence_parallel needs an Open-Sora forward installed (init_magcache_opensora / init_teacache_opensora)")
+    if any(k in model.__dict__ for k in ENGINE_ATTRS):
+        raise RuntimeError("enable_sequence_parallel must be called before the first forward")
+    if not 0 <= rank < world:
+        raise ValueError(f"enable_sequence_parallel: rank {rank} outside a world of {world}")
+    object.__setattr__(model, "_mc_sp_kw", dict(sp_world=world, sp_rank=rank, sp_group=group))
     return model
 
 
@@ -521,7 +540,8 @@ def _opensora_unsupported(self, x_mask, kw):
         raise NotImplementedError("magcache_b200: Open-Sora x_mask (image / video conditioning with t0) is not supported")
     pm = getattr(self, "parallel_manager", None)
     if pm is not None and (getattr(pm, "sp_size", 1) > 1 or getattr(pm, "cp_size", 1) > 1):
-        raise NotImplementedError("magcache_b200: Open-Sora sequence / CFG parallelism (sp_size or cp_size > 1) is not supported")
+        raise NotImplementedError("magcache_b200: VideoSys's own Open-Sora sequence / CFG parallelism (sp_size or cp_size > 1) is not "
+                                  "supported; keep sp_size = cp_size = 1 and call magcache_b200.enable_sequence_parallel")
     try:
         from videosys.core.pab_mgr import enable_pab
         pab = enable_pab()
@@ -535,7 +555,8 @@ def _opensora_unsupported(self, x_mask, kw):
 
 def opensora_engine(self, device):
     """The Open-Sora engine cached on the module, built on `device` at first use."""
-    return _cached_engine(self, "_mc_opensora_engine", lambda **skw: OpenSoraEngine(OpenSoraWeights.from_module(self, device), **skw))
+    sp = self.__dict__.get("_mc_sp_kw", {})  # enable_sequence_parallel
+    return _cached_engine(self, "_mc_opensora_engine", lambda **skw: OpenSoraEngine(OpenSoraWeights.from_module(self, device), **skw, **sp))
 
 
 def _opensora_stage(self, x, timestep, y, mask, x_mask, fps, height, width, kw):
@@ -554,7 +575,8 @@ def magcache_opensora_forward(self, x, timestep, all_timesteps, y, mask=None, x_
     (:349-354) and the skip line of :312 is printed. `residual_cache` is the engine's one residual buffer viewed as (B, N, C, 1): the
     reference's depth-3 FIFO is only ever read at [..., -1]; a tensor the caller puts there is honoured through its [..., -1].
     Cross-attention follows `flash_attn_varlen_func`: each sample attends to its own `y_lens[b]` caption tokens (the default
-    `torch_impl` agrees whenever the lengths are equal, as for one prompt's CFG pair)."""
+    `torch_impl` agrees whenever the lengths are equal, as for one prompt's CFG pair). Under `enable_sequence_parallel` the cache is
+    sharded as in the reference (:342-347): `residual_cache` is (B, N_r, C, 1), this rank's frames."""
     eng = _opensora_stage(self, x, timestep, y, mask, x_mask, fps, height, width, kw)
     skip_forward = self.t >= self.skip_time and _ctrl(self, "opensora").decide(self)  # :297-308
     cur = self.residual_cache
@@ -596,7 +618,10 @@ def teacache_opensora_forward(self, x, timestep, all_timesteps, y, mask=None, x_
     same tensor to block 0's qkv projection. A call is forced when `timestep[0]` (rounded to bf16) equals the first or the last of
     `all_timesteps`; there is no counter and nothing is reset between videos. `previous_modulated_input` / `previous_residual` are
     views of the engine's buffers, (B, N, C); a tensor the caller puts there is honoured. With `enable_teacache` False the call is the
-    plain forward (`eval_base`). Unsupported inputs raise as in `magcache_opensora_forward`."""
+    plain forward (`eval_base`). Unsupported inputs raise as in `magcache_opensora_forward`. Under `enable_sequence_parallel` the
+    decision input still covers every row on every rank (the reference forms it before its split), but `previous_residual` is
+    (B, N_r, C), this rank's frames: the reference gathers it to full size (:199-209) only to add its own frames back after the split,
+    so keeping it sharded changes no output."""
     eng = _opensora_stage(self, x, timestep, y, mask, x_mask, fps, height, width, kw)
     if not self.enable_teacache:  # :157-197
         return eng.forward_plain()
@@ -609,7 +634,7 @@ def teacache_opensora_forward(self, x, timestep, all_timesteps, y, mask=None, x_
     sums = eng.modulated_input(distance=not forced)
     rel = None if forced else opensora_rel_l1(sums[0], sums[1], eng.R * eng.w.dim)
     calc = _TEA_OS.decide(self, forced, rel)  # :96-107
-    self.previous_modulated_input = eng.mi[eng.mi_prev].view(eng.B, eng.N, -1)  # :108
+    self.previous_modulated_input = eng.mi[eng.mi_prev].view(eng.B, -1, eng.w.dim)  # :108 (every row, also under sequence parallelism)
     if not calc:
         cur = self.previous_residual
         _take_residual(eng, cur.reshape(eng.res.shape) if torch.is_tensor(cur) else cur)

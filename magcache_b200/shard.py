@@ -318,3 +318,248 @@ class P2PExchange:
 def make_exchange(shard, width, out_shape, device, extra_rows=0):
     use_p2p = torch.device(device).type == "cuda" and os.environ.get("MC_SHARD_P2P", "1") != "0"
     return (P2PExchange if use_p2p else CollectiveExchange)(shard, width, out_shape, device, extra_rows=extra_rows)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Open-Sora sequence parallelism (VideoSys DSP): frames for the spatial blocks, positions for the temporal blocks
+# ---------------------------------------------------------------------------------------------------------------------
+def frame_position_shards(world, T, S, group=None):
+    """The partition of `split_sequence` / `all_to_all_with_pad` (videosys/core/comm.py:297-381, `set_pad`): T frames (and S positions
+    per frame) padded up to a multiple of P and split in equal blocks, so rank r owns frames [r ceil(T/P), min((r+1) ceil(T/P), T))
+    and positions likewise. Returns ([TokenShard over T] * P, [TokenShard over S] * P). Pad frames / positions are never stored or
+    computed. A world that leaves a rank without a real frame (or position) raises ValueError: the reference would run that rank on
+    pad rows only."""
+    for what, n in (("T", T), ("S", S)):
+        if n < 1 or -(-n // world) * (world - 1) >= n:
+            raise ValueError(f"Open-Sora sequence parallelism: {what} = {n} {'latent frames' if what == 'T' else 'positions per frame'} on "
+                             f"P = {world} ranks leaves rank {world - 1} without a real {'frame' if what == 'T' else 'position'}")
+    return [TokenShard(r, world, T, group) for r in range(world)], [TokenShard(q, world, S, group) for q in range(world)]
+
+
+def _ceil256(n):
+    return (n + 255) // 256 * 256
+
+
+class _SwitchBase:
+    """Rows are `B (T S) D`. The frame-sharded layout of rank r holds, per sample b, frames [t0_r, t1_r) of every position:
+    row b T_r S + (t - t0_r) S + s. The position-sharded layout of rank q holds every frame of positions [s0_q, s1_q): row
+    b T S_q + t S_q + (s - s0_q) — itself `B (T S_q)`, so the temporal kernels run on it with S_q in place of S. One block of the
+    switch is, per (sample, peer), T_r strided runs of S_q rows (pitch S D) on the frame side and one contiguous run of T_r S_q rows
+    on the position side."""
+
+    def __init__(self, rank, world, B, T, S, D, Hx, Wx, device, group):
+        self.rank, self.world, self.group, self.device = rank, world, group, device
+        self.B, self.T, self.S, self.D, self.plane = B, T, S, D, Hx * Wx
+        self.frames, self.positions = frame_position_shards(world, T, S, group)
+        self.fr, self.ps = self.frames[rank], self.positions[rank]
+        self.out_shapes = {False: (B, 8, T, Hx, Wx), True: (B // 2, 4, T, Hx, Wx)}
+
+    def bytes_per_switch(self):
+        """bf16 bytes this rank sends to its peers in one switch (forward or backward; the two are equal)."""
+        return sum(self.B * self.fr.n_local * q.n_local * self.D * 2 for q in self.positions if q.rank != self.rank)
+
+
+class CollectiveSwitch(_SwitchBase):
+    """`all_to_all_single` over packed per-peer chunks for the switch and `all_gather` of padded frame windows for the output (gloo on
+    CPU in the test-suite; NCCL on the GPU with MC_SHARD_P2P=0)."""
+
+    p2p = False
+
+    def __init__(self, rank, world, B, T, S, D, Hx, Wx, device, group=None):
+        super().__init__(rank, world, B, T, S, D, Hx, Wx, device, group)
+        bf = dict(dtype=torch.bfloat16, device=device)
+        self.pos = torch.empty(B * T * self.ps.n_local, D, **bf)
+        self.frm = torch.empty(B * self.fr.n_local * S, D, **bf)
+        self.out = {k: torch.empty(v, dtype=torch.float32, device=device) for k, v in self.out_shapes.items()}
+
+    def _a2a(self, send, recv_sizes):
+        """One all_to_all_single of the bit patterns, as int32 pairs of bf16 (gloo has no 16-bit types; D is even)."""
+        send = [c.reshape(-1).view(torch.int32) for c in send]
+        recv = torch.empty(sum(recv_sizes) // 2, dtype=torch.int32, device=self.device)
+        dist.all_to_all_single(recv, torch.cat(send), output_split_sizes=[n // 2 for n in recv_sizes],
+                               input_split_sizes=[c.numel() for c in send], group=self.group)
+        return recv.view(torch.bfloat16).split(recv_sizes)
+
+    def to_positions(self, h):
+        """Frame-sharded [B T_r S, D] -> position-sharded [B T S_r, D] (dynamic_switch before the temporal attention)."""
+        B, S, D, fr, ps = self.B, self.S, self.D, self.fr, self.ps
+        hv = h.view(B, fr.n_local, S, D)
+        got = self._a2a([hv[:, :, q.start:q.stop] for q in self.positions], [B * p.n_local * ps.n_local * D for p in self.frames])
+        pv = self.pos.view(B, self.T, ps.n_local, D)
+        for p, c in zip(self.frames, got):
+            pv[:, p.start:p.stop].copy_(c.view(B, p.n_local, ps.n_local, D))
+        return self.pos
+
+    def to_frames(self, a):
+        """Position-sharded [B T S_r, D] -> frame-sharded [B T_r S, D] (dynamic_switch after the temporal attention)."""
+        B, S, D, fr, ps = self.B, self.S, self.D, self.fr, self.ps
+        av = a.view(B, self.T, ps.n_local, D)
+        got = self._a2a([av[:, p.start:p.stop] for p in self.frames], [B * fr.n_local * q.n_local * D for q in self.positions])
+        fv = self.frm.view(B, fr.n_local, S, D)
+        for q, c in zip(self.positions, got):
+            fv[:, :, q.start:q.stop].copy_(c.view(B, fr.n_local, q.n_local, D))
+        return self.frm
+
+    def output_buffer(self, step):
+        return self.out[step]
+
+    def gather_output(self, buf, out=None):
+        """Every rank wrote its frame window of `buf`; return the whole tensor on every rank (into `out` when given)."""
+        lead = buf.shape[0] * buf.shape[1]
+        n = self.fr.n_slots * self.plane
+        v = buf.view(lead, self.T * self.plane)
+        mine = torch.zeros(lead, n, dtype=torch.float32, device=self.device)
+        mine[:, :self.fr.n_local * self.plane] = v[:, self.fr.start * self.plane:self.fr.stop * self.plane]
+        parts = [torch.empty_like(mine) for _ in range(self.world)]
+        dist.all_gather(parts, mine, group=self.group)
+        res = torch.empty_like(buf) if out is None else out
+        rv = res.view(lead, self.T * self.plane)
+        for p, c in zip(self.frames, parts):
+            rv[:, p.start * self.plane:p.stop * self.plane] = c[:, :p.n_local * self.plane]
+        return res
+
+    def close(self):
+        pass
+
+
+class P2PSwitch(_SwitchBase):
+    """The switch and the output assembly on the copy engines (`mc_p2p_push2d`). Every rank owns one IPC window: flags, two
+    position-sharded receive buffers, two frame-sharded receive buffers and two full-size output slots. Exchange n of a direction
+    uses buffer n % 2 (DESIGN §7 argues why two are enough). All pushes run on the calling stream in the order of the forward, so
+    the stream that issued them is also the one that may overwrite their source; a one-block kernel (`mc_p2p_wait`) holds the
+    stream until every peer's flag has reached the exchange's epoch. No SM moves data. Constructed collectively."""
+
+    p2p = True
+    FLAG_BYTES = 4096
+
+    def __init__(self, rank, world, B, T, S, D, Hx, Wx, device, group=None):
+        super().__init__(rank, world, B, T, S, D, Hx, Wx, device, group)
+        from . import _lib
+        self._lib = _lib
+        lib, check = _lib.lib, _lib.check
+        assert world <= 64, "flag table: 64 entries per buffer"
+        s_slots, t_slots = self.positions[0].n_slots, self.frames[0].n_slots
+        self.pos_bytes = _ceil256(B * T * s_slots * D * 2)
+        self.frm_bytes = _ceil256(B * t_slots * S * D * 2)
+        self.out_bytes = _ceil256(B * 8 * T * self.plane * 4)
+        self.off_pos = [self.FLAG_BYTES + i * self.pos_bytes for i in range(2)]
+        self.off_frm = [self.FLAG_BYTES + 2 * self.pos_bytes + i * self.frm_bytes for i in range(2)]
+        self.off_out = [self.FLAG_BYTES + 2 * self.pos_bytes + 2 * self.frm_bytes + i * self.out_bytes for i in range(2)]
+        total = self.off_out[1] + self.out_bytes
+        ptr, handle = ctypes.c_void_p(), ctypes.create_string_buffer(64)
+        check(lib.mc_p2p_alloc(total, ctypes.byref(ptr), handle))
+        self.base = ptr.value
+        handles = [None] * world
+        dist.all_gather_object(handles, bytes(handle.raw), group=group)
+        self.peer_base = []
+        for r in range(world):
+            if r == rank:
+                self.peer_base.append(self.base)
+                continue
+            pp = ctypes.c_void_p()
+            check(lib.mc_p2p_open(ctypes.create_string_buffer(handles[r], 64), ctypes.byref(pp)))
+            self.peer_base.append(pp.value)
+        self.window = torch.as_tensor(_RawCuda(self.base, total), device=device)
+        self.flags = self.window[:self.FLAG_BYTES].view(torch.int32)  # [direction 0..2][parity][source rank] at 128 d + 64 parity + r
+        w = self.window
+
+        def view(off, rows, cols, dtype, nbytes):
+            return w[off:off + nbytes].view(dtype).view(rows, cols)
+
+        self.pos = [view(o, B * T * self.ps.n_local, D, torch.bfloat16, B * T * self.ps.n_local * D * 2) for o in self.off_pos]
+        self.frm = [view(o, B * self.fr.n_local * S, D, torch.bfloat16, B * self.fr.n_local * S * D * 2) for o in self.off_frm]
+        self.epochs = torch.zeros(4, dtype=torch.int32, device=device)  # [0] forward switch, [1] backward switch, [2] output
+        self.count = [0, 0, 0]
+        # push order: the nearest peers first (r + 1, r - 1, r + 2, ...), this rank's own block last
+        near = sorted((q for q in range(world) if q != rank), key=lambda q: (min((q - rank) % world, (rank - q) % world), (q - rank) % world))
+        self.order = near + [rank]
+        dist.barrier(group=group)  # every window is mapped before anyone pushes
+
+    def _flag(self, r, d, parity, src):
+        return self.peer_base[r] + 4 * (128 * d + 64 * parity + src)
+
+    def _exchange(self, d, copies):
+        """Round of direction d: bump its epoch (this rank's own flag with it), issue `copies` [(dst, dpitch, src, spitch, width,
+        height)], one flag per peer, then wait on the stream for every rank's flag. Returns the parity used."""
+        lib, check = self._lib.lib, self._lib.check
+        i = self.count[d] % 2
+        self.count[d] += 1
+        stream = torch.cuda.current_stream().cuda_stream
+        ep = self.epochs[d:d + 1]
+        own = self.flags[128 * d + 64 * i:128 * d + 64 * i + self.world]
+        check(lib.mc_p2p_bump(ep.data_ptr(), own[self.rank:self.rank + 1].data_ptr(), stream))
+        arr = (self._lib.Copy2D * len(copies))(*[self._lib.Copy2D(*c) for c in copies])
+        peers = [q for q in self.order if q != self.rank]
+        flg = (ctypes.c_void_p * len(peers))(*[self._flag(q, d, i, self.rank) for q in peers])
+        check(lib.mc_p2p_push2d(arr, len(copies), flg, len(peers), ep.data_ptr(), stream))
+        check(lib.mc_p2p_wait(own.data_ptr(), self.world, ep.data_ptr(), stream))
+        return i
+
+    def _blocks(self, parity, forward, src):
+        B, T, S, D, fr = self.B, self.T, self.S, self.D, self.fr
+        i, copies = parity, []
+        for q in self.order:
+            pq = self.positions[q]
+            for b in range(B):
+                frame_side = src if forward else self.peer_base[q] + self.off_frm[i]
+                frame_off = (b * fr.n_local * S + pq.start) * D * 2 if forward else (b * self.frames[q].n_local * S + self.ps.start) * D * 2
+                if forward:  # this rank's frames, positions of q -> q's position buffer
+                    copies.append((self.peer_base[q] + self.off_pos[i] + (b * T * pq.n_local + fr.start * pq.n_local) * D * 2,
+                                   pq.n_local * D * 2, frame_side + frame_off, S * D * 2, pq.n_local * D * 2, fr.n_local))
+                else:        # every frame of this rank's positions: q's frames -> q's frame buffer
+                    fq = self.frames[q]
+                    copies.append((frame_side + frame_off, S * D * 2,
+                                   src + (b * T * self.ps.n_local + fq.start * self.ps.n_local) * D * 2, self.ps.n_local * D * 2,
+                                   self.ps.n_local * D * 2, fq.n_local))
+        return copies
+
+    def to_positions(self, h):
+        assert h.is_contiguous() and h.shape == (self.B * self.fr.n_local * self.S, self.D)
+        i = self.count[0] % 2
+        self._exchange(0, self._blocks(i, True, h.data_ptr()))
+        return self.pos[i]
+
+    def to_frames(self, a):
+        assert a.is_contiguous() and a.shape == (self.B * self.T * self.ps.n_local, self.D)
+        i = self.count[1] % 2
+        self._exchange(1, self._blocks(i, False, a.data_ptr()))
+        return self.frm[i]
+
+    def output_buffer(self, step):
+        i = self.count[2] % 2
+        shape = self.out_shapes[step]
+        n = 1
+        for v in shape:
+            n *= v
+        return self.window[self.off_out[i]:self.off_out[i] + 4 * n].view(torch.float32).view(shape)
+
+    def gather_output(self, buf, out=None):
+        """This rank's frame window of `buf` (the current output slot) into the same slot of every peer: height (samples x channels),
+        width T_r Hx Wx fp32, pitch T Hx Wx. Then the whole tensor is copied out of the window (it is rewritten two outputs later)."""
+        i = self.count[2] % 2
+        assert buf.data_ptr() == self.base + self.off_out[i]
+        lead, fr, pl = buf.shape[0] * buf.shape[1], self.fr, self.plane
+        off = fr.start * pl * 4
+        copies = [(self.peer_base[q] + self.off_out[i] + off, self.T * pl * 4, self.base + self.off_out[i] + off, self.T * pl * 4,
+                   fr.n_local * pl * 4, lead) for q in self.order if q != self.rank]
+        self._exchange(2, copies)
+        if out is None:
+            return buf.clone()
+        return out.copy_(buf)
+
+    def close(self):
+        lib = self._lib.lib
+        torch.cuda.synchronize()
+        for r, pb in enumerate(self.peer_base):
+            if r != self.rank and pb:
+                lib.mc_p2p_close(pb)
+        self.peer_base = []
+        self.window = self.pos = self.frm = None
+        if self.base:
+            lib.mc_p2p_free(self.base)
+            self.base = 0
+
+
+def make_switch(rank, world, B, T, S, D, Hx, Wx, device, group=None):
+    use_p2p = torch.device(device).type == "cuda" and os.environ.get("MC_SHARD_P2P", "1") != "0"
+    return (P2PSwitch if use_p2p else CollectiveSwitch)(rank, world, B, T, S, D, Hx, Wx, device, group)
