@@ -334,13 +334,20 @@ def test_shape_table_matches_the_engines():
 
 
 # ------------------------------------------------------------------------------------------- (a) one-layer forwards
+def rule_fraction(out, ref, exact):
+    """DESIGN §5's rule without the assertion: (e_ref, e_ours, e_vs, the larger of the two errors as a fraction of its bound).
+    The rule holds exactly when the fraction is <= 1."""
+    e_ref, e_vs, e_ours = rel_l2(ref, exact), rel_l2(out, ref), rel_l2(out, exact)
+    return e_ref, e_ours, e_vs, max(e_vs / (2.0 * e_ref + 1e-3), e_ours / (1.5 * e_ref + 1e-3))
+
+
 def _rule(what, out, ref, exact, verbose=True):
     """DESIGN §5's rule; returns the larger of its two errors as a fraction of its bound."""
-    e_ref, e_vs, e_ours = rel_l2(ref, exact), rel_l2(out, ref), rel_l2(out, exact)
+    e_ref, e_ours, e_vs, frac = rule_fraction(out, ref, exact)
     if verbose:
         print(f"  {what}: ours vs fp64 {e_ours:.3e} | oracle(bf16) vs fp64 {e_ref:.3e} | ours vs oracle {e_vs:.3e}")
     assert e_vs <= 2.0 * e_ref + 1e-3 and e_ours <= 1.5 * e_ref + 1e-3, (what, e_ours, e_ref, e_vs)
-    return max(e_vs / (2.0 * e_ref + 1e-3), e_ours / (1.5 * e_ref + 1e-3))
+    return frac
 
 
 def _forward_loop(name, calls, ours, ref_m, m64, exact_ctx, res_attr, attrs, check=None):

@@ -16,7 +16,8 @@ def rel_l2(a, b):
 
 
 @pytest.mark.parametrize("dims_kw,grid", [(dict(dim=256, ffn_dim=512, num_heads=2, num_layers=2), (3, 16, 24)),
-                                           (dict(dim=1536, ffn_dim=8960, num_heads=12, num_layers=1), (3, 30, 52))])
+                                           (dict(dim=1536, ffn_dim=8960, num_heads=12, num_layers=1), (3, 30, 52)),
+                                           (dict(dim=1536, ffn_dim=8960, num_heads=12, num_layers=30), (21, 30, 52))])
 def test_native_forward_bit_equal_to_python_sequenced(dims_kw, grid):
     import magcache_b200 as mc
     from magcache_b200 import ops
