@@ -308,6 +308,18 @@ int32_t mc_silu_bf16(const void* x, void* y, int64_t n, void* stream);
 #define MC_EPI_BIAS_SILU_BF16 7   /* out_bf16 = bf16(silu(float(bf16(acc + bias[n]))))                 TimestepEmbedding linear_1 + SiLU */
 int32_t mc_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t M, int32_t N, int32_t K,
                      const float* bias, int32_t epilogue, void* out, int64_t ldo, const float* gate, void* stream);
+/* MC_EPI_BIAS_GATE_RESID_ADD_BF16 (mc_gemm_bf16_add only; mc_gemm_bf16 rejects it): epilogue 6, then a bf16 addend on the rows
+ * m >= add_row0 — a FLUX ControlNet residual after a block (`hidden_states = hidden_states + controlnet_block_samples[...]`,
+ * MagCache4FLUX/magcache_flux.py:374-384; single blocks on the image rows only, :416-423):
+ *   y   = bf16(acc + bias[n])
+ *   x1  = bf16(x[m,n] + bf16(gate[n] * y))                          what epilogue 6 writes
+ *   out = m >= add_row0 ? bf16(x1 + add[(m - add_row0) * ld_add + n]) : x1
+ * Rows below add_row0 neither read the addend nor add 0 to it (a -0 stays -0): they are bit-identical to epilogue 6. The addend is
+ * read only inside [add_row0, M) x [0, N); any ld_add >= N and any 2-byte-aligned base are accepted (0 <= add_row0 < M). */
+#define MC_EPI_BIAS_GATE_RESID_ADD_BF16 8
+int32_t mc_gemm_bf16_add(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t M, int32_t N, int32_t K,
+                         const float* bias, void* out, int64_t ldo, const float* gate, const void* add, int64_t ld_add, int32_t add_row0,
+                         void* stream);
 
 /* Non-causal attention forward on wgmma: out[i, h*128:(h+1)*128] = softmax(q_h k_h^T * scale) v_h, head_dim = 128
  * (WanSelfAttention / WanT2VCrossAttention [EXT] behind MagCache4Wan2.1/magcache_generate.py:297-298; the joint attention of

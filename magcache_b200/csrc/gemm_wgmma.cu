@@ -59,6 +59,9 @@ struct GemmParams {
   int64_t ldo;
   const float* gate;
   int total_tiles;  // 256-row m tiles x n tiles (cluster steps), set by launch_gemm_bn: read from the parameter bank
+  const __nv_bfloat16* add;  // MC_EPI_BIAS_GATE_RESID_ADD_BF16 only: addend rows [add_row0, M), row stride ld_add
+  int64_t ld_add;
+  int add_row0;
 };
 
 // One ROWS-row x 32-column patch: `stage` holds acc[r][c] at stage[r*33 + c]; lane = column. All global accesses below
@@ -67,6 +70,8 @@ template <int EPI, int ROWS>
 __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float* stage, int row0, int col0, int lane) {
   const int rows = min(ROWS, p.M - row0);
   if (rows <= 0) return;
+  constexpr bool kAdd = EPI == MC_EPI_BIAS_GATE_RESID_ADD_BF16;
+  constexpr bool kGateResidBf16 = EPI == MC_EPI_BIAS_GATE_RESID_BF16 || kAdd;  // epilogue 8 is epilogue 6, then the addend
   const int col = col0 + lane;
   const bool col_ok = col < p.N;
 
@@ -111,7 +116,7 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
     if (c0 + 1 < p.N) b1 = p.bias[c0 + 1];
   }
   float g0 = 1.f, g1 = 1.f;
-  if (EPI == MC_EPI_BIAS_GATE_RESID_BF16 && p.gate) {
+  if (kGateResidBf16 && p.gate) {
     if (c0 < p.N) g0 = p.gate[c0];
     if (c0 + 1 < p.N) g1 = p.gate[c0 + 1];
   }
@@ -119,7 +124,11 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
   const float* sbase = stage + half * kStagePad + cp;
   const float* rbias = (EPI == MC_EPI_ROWBIAS_BF16 && p.bias) ? p.bias + row0 + half : nullptr;
 
-  if (rows == ROWS && col0 + 32 <= p.N && (p.ldo & 1) == 0) {
+  // epilogue 8: the patch lies wholly at or past add_row0 (every row adds) or wholly before it (none reads the addend)
+  const bool add_rows = kAdd && row0 >= p.add_row0;
+  const bool add_uniform = !kAdd || row0 + ROWS <= p.add_row0 ||
+                           (add_rows && (p.ld_add & 1) == 0 && (reinterpret_cast<uintptr_t>(p.add) & 3u) == 0);
+  if (rows == ROWS && col0 + 32 <= p.N && (p.ldo & 1) == 0 && add_uniform) {
     // interior patch: branch-free, ROWS / 2 independent iterations for the scheduler to interleave
     uint32_t w[ROWS / 2];
 #pragma unroll
@@ -145,12 +154,20 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
         v0 = silu_f(round_bf16(v0));
         v1 = silu_f(round_bf16(v1));
       }
-      if (EPI == MC_EPI_BIAS_GATE_RESID_BF16) {  // x = x + g * y with every tensor bf16 (MMDiT streams): three roundings
+      if (kGateResidBf16) {  // x = x + g * y with every tensor bf16 (MMDiT streams): three roundings
         const uint32_t old = *reinterpret_cast<const uint32_t*>(obase + static_cast<int64_t>(2 * i) * p.ldo);
         v0 = bf16_lo(old) + round_bf16(g0 * round_bf16(v0));
         v1 = bf16_hi(old) + round_bf16(g1 * round_bf16(v1));
       }
       w[i] = pack_bf16x2(v0, v1);
+    }
+    if (add_rows) {  // out = bf16(x1 + add): the second rounding, on the bf16 x1 just packed (32-bit pairs, like the `old` loads)
+      const __nv_bfloat16* abase = p.add + static_cast<int64_t>(row0 + half - p.add_row0) * p.ld_add + c0;
+#pragma unroll
+      for (int i = 0; i < ROWS / 2; ++i) {
+        const uint32_t a = *reinterpret_cast<const uint32_t*>(abase + static_cast<int64_t>(2 * i) * p.ld_add);
+        w[i] = pack_bf16x2(bf16_lo(w[i]) + bf16_lo(a), bf16_hi(w[i]) + bf16_hi(a));
+      }
     }
 #pragma unroll
     for (int i = 0; i < ROWS / 2; ++i) *reinterpret_cast<uint32_t*>(obase + static_cast<int64_t>(2 * i) * p.ldo) = w[i];
@@ -183,9 +200,14 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
       v1 = silu_f(round_bf16(v1));
     }
     __nv_bfloat16* o = obase + static_cast<int64_t>(2 * i) * p.ldo;
-    if (EPI == MC_EPI_BIAS_GATE_RESID_BF16) {
+    if (kGateResidBf16) {
       if (c0 < p.N) v0 = __bfloat162float(o[0]) + round_bf16(g0 * round_bf16(v0));
       if (c0 + 1 < p.N) v1 = __bfloat162float(o[1]) + round_bf16(g1 * round_bf16(v1));
+    }
+    if (kAdd && row0 + r >= p.add_row0) {  // scalar loads: ragged rows / columns, odd ld_add, 2-byte-aligned addend
+      const __nv_bfloat16* a = p.add + static_cast<int64_t>(row0 + r - p.add_row0) * p.ld_add + c0;
+      if (c0 < p.N) v0 = round_bf16(v0) + __bfloat162float(a[0]);
+      if (c0 + 1 < p.N) v1 = round_bf16(v1) + __bfloat162float(a[1]);
     }
     if (pair_ok) {
       *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(v0, v1);
@@ -386,24 +408,30 @@ static int pick_bn(int M, int N) {
   return cost128 * 100 <= cost256 * 92 ? 128 : 256;
 }
 
+// The argument checks and tensor maps every GEMM entry point shares; `fn` names the entry point in the error text.
+static int32_t gemm_prepare(const char* fn, const void* A, int64_t lda, const void* B, int64_t ldb, int32_t M, int32_t N, int32_t K,
+                            const void* out, int64_t ldo, CUtensorMap* ta, CUtensorMap* tb, int* bn) {
+  MC_CHECK_ARG(A && B && out, "%s: null pointer", fn);
+  MC_CHECK_ARG(M >= 1 && N >= 1 && K >= 8, "%s: M=%d N=%d K=%d", fn, M, N, K);
+  MC_CHECK_ARG(K % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0 && lda >= K && ldb >= K, "%s: K/lda/ldb must be multiples of 8 (16-byte TMA pitch)", fn);
+  MC_CHECK_ARG(aligned16(A) && aligned16(B) && aligned16(out), "%s: A/B/out must be 16-byte aligned", fn);
+  MC_CHECK_ARG(ldo >= N, "%s: ldo=%lld < N=%d", fn, static_cast<long long>(ldo), N);
+  int32_t rc = make_tmap_bf16_2d(ta, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(lda), kBM, kBK);
+  if (rc) return rc;
+  *bn = pick_bn(M, N);
+  // each CTA of a cluster loads (and multicasts) one half of the B tile: the box is bn / 2 rows
+  return make_tmap_bf16_2d(tb, B, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), *bn / kCluster, kBK);
+}
+
 }  // namespace mc
 
 extern "C" int32_t mc_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t M, int32_t N, int32_t K,
                                 const float* bias, int32_t epilogue, void* out, int64_t ldo, const float* gate, void* stream) {
-  MC_CHECK_ARG(A && B && out, "mc_gemm_bf16: null pointer");
-  MC_CHECK_ARG(M >= 1 && N >= 1 && K >= 8, "mc_gemm_bf16: M=%d N=%d K=%d", M, N, K);
-  MC_CHECK_ARG(K % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0 && lda >= K && ldb >= K, "mc_gemm_bf16: K/lda/ldb must be multiples of 8 (16-byte TMA pitch)");
-  MC_CHECK_ARG(mc::aligned16(A) && mc::aligned16(B) && mc::aligned16(out), "mc_gemm_bf16: A/B/out must be 16-byte aligned");
-  MC_CHECK_ARG(ldo >= N, "mc_gemm_bf16: ldo=%lld < N=%d", static_cast<long long>(ldo), N);
   CUtensorMap ta, tb;
-  int32_t rc = mc::make_tmap_bf16_2d(&ta, A, static_cast<uint64_t>(M), static_cast<uint64_t>(K), static_cast<uint64_t>(lda), mc::kBM, mc::kBK);
+  int bn = 0;
+  const int32_t rc = mc::gemm_prepare("mc_gemm_bf16", A, lda, B, ldb, M, N, K, out, ldo, &ta, &tb, &bn);
   if (rc) return rc;
-  const int bn = mc::pick_bn(M, N);
-  // each CTA of a cluster loads (and multicasts) one half of the B tile: the box is bn / 2 rows
-  rc = mc::make_tmap_bf16_2d(&tb, B, static_cast<uint64_t>(N), static_cast<uint64_t>(K), static_cast<uint64_t>(ldb), bn / mc::kCluster,
-                             mc::kBK);
-  if (rc) return rc;
-  mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0};
+  mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0, nullptr, 0, 0};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 #define MC_GEMM_CASE(E) \
   case E: return bn == 128 ? mc::launch_gemm_bn<E, 128>(ta, tb, p, s) : mc::launch_gemm_bn<E, 256>(ta, tb, p, s)
@@ -421,4 +449,20 @@ extern "C" int32_t mc_gemm_bf16(const void* A, int64_t lda, const void* B, int64
       mc::set_error("mc_gemm_bf16: unknown epilogue %d", epilogue);
       return MC_ERR_INVALID;
   }
+}
+
+extern "C" int32_t mc_gemm_bf16_add(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t M, int32_t N, int32_t K,
+                                    const float* bias, void* out, int64_t ldo, const float* gate, const void* add, int64_t ld_add,
+                                    int32_t add_row0, void* stream) {
+  CUtensorMap ta, tb;
+  int bn = 0;
+  const int32_t rc = mc::gemm_prepare("mc_gemm_bf16_add", A, lda, B, ldb, M, N, K, out, ldo, &ta, &tb, &bn);
+  if (rc) return rc;
+  MC_CHECK_ARG(add, "mc_gemm_bf16_add: null addend");
+  MC_CHECK_ARG(ld_add >= N, "mc_gemm_bf16_add: ld_add=%lld < N=%d", static_cast<long long>(ld_add), N);
+  MC_CHECK_ARG(add_row0 >= 0 && add_row0 < M, "mc_gemm_bf16_add: add_row0=%d outside [0, M=%d)", add_row0, M);
+  const mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0, static_cast<const __nv_bfloat16*>(add), ld_add, add_row0};
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  return bn == 128 ? mc::launch_gemm_bn<MC_EPI_BIAS_GATE_RESID_ADD_BF16, 128>(ta, tb, p, s)
+                   : mc::launch_gemm_bn<MC_EPI_BIAS_GATE_RESID_ADD_BF16, 256>(ta, tb, p, s);
 }

@@ -62,12 +62,16 @@ class Fp8Weight:
         return Fp8Weight(self.q[rows], self.scale[rows])
 
 
-def linear(a, w, bias, epilogue, out, gate=None, scratch=None):
-    """`ops.gemm(a, w, ...)` for a bf16 weight. For an Fp8Weight: per block of rows that fits `scratch` (bf16), one
-    `dequant_fp8_bf16` into the scratch, then the unchanged bf16 GEMM on it for the matching output columns. Every epilogue but
-    MC_EPI_ROWBIAS_BF16 is column-wise, so the blocks compute exactly the columns one GEMM would."""
+def linear(a, w, bias, epilogue, out, gate=None, scratch=None, addend=None, addend_row0=0):
+    """`ops.gemm(a, w, ...)` for a bf16 weight (with an `addend`: the ControlNet epilogue, see ops.gemm). For an Fp8Weight: per
+    block of rows that fits `scratch` (bf16), one `dequant_fp8_bf16` into the scratch, then the unchanged bf16 GEMM on it for the
+    matching output columns. Every epilogue but MC_EPI_ROWBIAS_BF16 is column-wise, so the blocks compute exactly the columns one
+    GEMM would."""
     if not isinstance(w, Fp8Weight):
-        return ops.gemm(a, w, bias, epilogue, out=out, gate=gate)
+        if addend is None:
+            return ops.gemm(a, w, bias, epilogue, out=out, gate=gate)
+        return ops.gemm(a, w, bias, epilogue, out=out, gate=gate, addend=addend, addend_row0=addend_row0)
+    assert addend is None, "no FP8 family has ControlNet residuals"
     assert epilogue != E.MC_EPI_ROWBIAS_BF16 and out is not None and scratch is not None
     rows, cols = w.shape
     step = max(8, scratch.numel() // cols // 8 * 8)  # multiples of 8 rows keep every output column block 16-byte aligned
@@ -159,11 +163,23 @@ def rope_table(ids, device, axes_dim=(16, 56, 56), theta=10000.0):
     return torch.tensor(cs.astype(np.float32)).to(device)  # torch-allocated (aligned) storage on every device
 
 
+def controlnet_index(i, n_blocks, n_samples, repeat=False):
+    """Index of the ControlNet sample added after block `i` of `n_blocks`: the reference's expressions (magcache_flux.py:376-384 for
+    the double blocks, `repeat` = XLabs' controlnet_blocks_repeat; :418-423 for the single blocks, which never repeat). The interval
+    is computed first, as there, so an empty sample list raises ZeroDivisionError either way."""
+    interval = int(np.ceil(n_blocks / n_samples))
+    return i % n_samples if repeat else i // interval
+
+
 class MMDiTCore:
     """Workspace + block stack shared by the FLUX and HunyuanVideo engines. A subclass provides `self.w` (dim, heads, double, single,
     ada_w / ada_b / ada_rows), the token order (`txt_first`), the RoPE table of the rows that get RoPE, and its own prologue / head."""
 
     txt_first = True
+
+    def _controlnet_views(self):
+        """`run_blocks`' ControlNet argument for the current call; only the FLUX engine takes ControlNet residuals."""
+        return None
 
     def _alloc_core(self, n_img, n_txt):
         """Buffers for one (image tokens, text tokens) shape. Token-sharded (`self.world > 1`, SURVEY §8e): the IMAGE rows are split over
@@ -223,9 +239,9 @@ class MMDiTCore:
                 self._linear(s, wt, w.ada_b[r0:r1], E.MC_EPI_BIAS_BF16, out=self.ada[:, r0:r1])
         ops.cast_into(self.ada.view(-1), self.adaf)
 
-    def _linear(self, a, wt, bias, epilogue, out, gate=None):
+    def _linear(self, a, wt, bias, epilogue, out, gate=None, addend=None, addend_row0=0):
         """A block Linear: bf16 or Fp8Weight (`linear`), through the weights' dequantisation scratch."""
-        return linear(a, wt, bias, epilogue, out, gate=gate, scratch=self.w.fp8_scratch)
+        return linear(a, wt, bias, epilogue, out, gate=gate, scratch=self.w.fp8_scratch, addend=addend, addend_row0=addend_row0)
 
     def _rope_for(self, rows):
         """RoPE table rows for a token range, or None when that range gets no RoPE (HunyuanVideo text tokens)."""
@@ -291,13 +307,19 @@ class MMDiTCore:
         gather_rows(o_local.contiguous(), full, self.shard.group)
         return full
 
-    def run_blocks(self):
+    def run_blocks(self, ctrl=None):
         """Double-stream then single-stream blocks (magcache_flux.py:343-424; magcache_sample_video.py:108-139) on `hs`; the image rows of
-        `hs` must hold the embedded image tokens and the text rows the embedded text. Returns the image rows."""
+        `hs` must hold the embedded image tokens and the text rows the embedded text. Returns the image rows.
+
+        `ctrl`: None, or (double, single) lists with one entry per block — a bf16 [n_img, D] view (this rank's image rows) added to
+        the image stream after that block (FLUX ControlNet residuals, magcache_flux.py:374-384 / :416-423), or None. The addition is
+        fused into the block's last GEMM on the image rows (MC_EPI_BIAS_GATE_RESID_ADD_BF16): FF2 of the image stream of a double
+        block, the `out` GEMM of a single block from row n_txt on (text rows first, FLUX only)."""
         w, D, S = self.w, self.w.dim, self.S
+        c_double, c_single = ctrl if ctrl is not None else ((None,) * len(w.double), (None,) * len(w.single))
         txt, img = self.txt, self.img
         hs, h = self.hs, self.h
-        for b in w.double:
+        for b, add in zip(w.double, c_double):
             em, emc = self._em(b["ada"], 6), self._em(b["ada_c"], 6)  # (shift1, scale1, gate1, shift2, scale2, gate2)
             ops.ln_modulate(hs[img], em, 1, 0, round_ln_to_bf16=True, out=h[img])
             ops.ln_modulate(hs[txt], emc, 1, 0, round_ln_to_bf16=True, out=h[txt])
@@ -313,9 +335,9 @@ class MMDiTCore:
                 ops.ln_modulate(hs[rows], e, 4, 3, round_ln_to_bf16=True, out=h[rows])
                 ffh = self.cat[rows][:, D:]
                 self._linear(h[rows], f1w, f1b, E.MC_EPI_BIAS_GELU_BF16, out=ffh)
-                self._linear(ffh, f2w, f2b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[rows], gate=e[5])
+                self._linear(ffh, f2w, f2b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[rows], gate=e[5], addend=add if rows == img else None)
         allr = slice(0, S)
-        for b in w.single:
+        for b, add in zip(w.single, c_single):
             em = self._em(b["ada"], 3)  # (shift, scale, gate)
             ops.ln_modulate(hs, em, 1, 0, round_ln_to_bf16=True, out=h)
             self._linear(h, b["mlp_w"], b["mlp_b"], E.MC_EPI_BIAS_GELU_BF16, out=self.cat[:, D:])
@@ -323,7 +345,8 @@ class MMDiTCore:
             self._qk_norm(img, b["nq"], b["nk"])
             self._qk_norm(txt, b["nq"], b["nk"])
             self._joint_attention(self.cat[:, :D])
-            self._linear(self.cat, b["out_w"], b["out_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs, gate=em[2])
+            self._linear(self.cat, b["out_w"], b["out_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs, gate=em[2], addend=add,
+                         addend_row0=self.n_txt)
         return hs[img]
 
     def _time_mlp(self, x_bf16, mlp):
@@ -344,7 +367,7 @@ class MMDiTCore:
             x = ops.cache_hit_add(x0, self.res, out=self.hit)                     # magcache_flux.py:340 ; magcache_sample_video.py:104
         else:
             self.hs[self.img].copy_(x0)                                           # `ori_hidden_states` / `ori_img` stays in x0
-            x = self.run_blocks()
+            x = self.run_blocks(self._controlnet_views())
             if self.shard is not None:
                 self.xch.join()  # every push of this forward is ordered before its end
             ops.residual_sub(x.contiguous(), x0, out=self.res)                    # :426 ; :140 (x is a contiguous row range of hs)
@@ -359,7 +382,7 @@ class MMDiTCore:
         multiples of 2^-8 (the shipped FLUX table is visibly bf16-quantised, SURVEY §8a row 9)."""
         x0 = self.prologue()
         self.hs[self.img].copy_(x0)
-        x = self.run_blocks()
+        x = self.run_blocks(self._controlnet_views())
         reduce = None
         if self.shard is not None:  # the statistics are sums over the image tokens: add the partial sums of every token shard
             from .shard import allreduce_stats
@@ -382,6 +405,7 @@ class FluxEngine(MMDiTCore):
         self._shape = None
         self._rope_key, self._rope = None, None
         self.res_valid = False
+        self.controlnet = (None, None, False)
 
     def _workspace(self, n_img, n_txt):
         if self._shape == (n_img, n_txt):
@@ -423,6 +447,39 @@ class FluxEngine(MMDiTCore):
             self._rope = rope_table(torch.cat((txt_ids.reshape(-1, 3), img_ids.reshape(-1, 3)), dim=0), self.device)  # :318
             self._rope_key = key
             assert self._rope.shape == (self.S_keys, 128)
+
+    def stage_controlnet(self, block_samples, single_block_samples, blocks_repeat=False):
+        """The call's ControlNet residuals (`controlnet_block_samples`, `controlnet_single_block_samples`,
+        `controlnet_blocks_repeat`). Kept as given: they are validated and read only when the block stack runs (a miss or a
+        calibration call); a hit ignores them, as the reference does."""
+        self.controlnet = (block_samples, single_block_samples, bool(blocks_repeat))
+
+    def _controlnet_sample(self, sample, what):
+        """This rank's rows of one sample as a [n_img, D] view (no copy). Only a CUDA bf16 [1, n_img, D] tensor with unit column
+        stride is taken: the reference's `hidden_states + sample` would broadcast other shapes and promote an fp32 sample, changing
+        the stream's dtype."""
+        want = (1, self.n_img_total, self.w.dim)
+        if not (torch.is_tensor(sample) and sample.is_cuda and sample.device == self.hs.device and sample.dtype == torch.bfloat16
+                and tuple(sample.shape) == want and sample.stride(-1) == 1):
+            got = (f"{sample.dtype} {tuple(sample.shape)} on {sample.device}" if torch.is_tensor(sample) else type(sample).__name__)
+            raise NotImplementedError(f"magcache_b200: {what} must be a bf16 CUDA tensor of shape {list(want)} with unit column stride "
+                                      f"on {self.hs.device}; got {got}")
+        return sample[0] if self.shard is None else sample[0, self.shard.start:self.shard.stop]
+
+    def _controlnet_views(self):
+        block_samples, single_samples, repeat = self.controlnet
+        if block_samples is None and single_samples is None:
+            return None
+        w = self.w
+        views = []
+        for samples, blocks, rep, name in ((block_samples, w.double, repeat, "controlnet_block_samples"),
+                                           (single_samples, w.single, False, "controlnet_single_block_samples")):
+            if samples is None:
+                views.append([None] * len(blocks))
+                continue
+            idx = [controlnet_index(i, len(blocks), len(samples), rep) for i in range(len(blocks))]
+            views.append([self._controlnet_sample(samples[j], f"{name}[{j}]") for j in idx])
+        return tuple(views)
 
     def prologue(self):
         """x_embedder, time_text_embed, context_embedder (:290-303) and every AdaLayerNorm projection of the forward."""

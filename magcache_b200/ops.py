@@ -448,8 +448,12 @@ def silu(x, out=None):
     return out
 
 
-def gemm(a, b, bias=None, epilogue=_lib.MC_EPI_BIAS_BF16, out=None, gate=None, tag=None):
-    """acc = a @ b.T on wgmma (a [M,K] bf16, b [N,K] bf16, row stride allowed) + fused epilogue (see MC_EPI_*)."""
+def gemm(a, b, bias=None, epilogue=_lib.MC_EPI_BIAS_BF16, out=None, gate=None, tag=None, addend=None, addend_row0=0):
+    """acc = a @ b.T on wgmma (a [M,K] bf16, b [N,K] bf16, row stride allowed) + fused epilogue (see MC_EPI_*).
+
+    `addend` (bf16 [M - addend_row0, N], unit column stride, row stride allowed) turns MC_EPI_BIAS_GATE_RESID_BF16 into
+    MC_EPI_BIAS_GATE_RESID_ADD_BF16 (`mc_gemm_bf16_add`): epilogue 6 in place on `out`, then
+    out[addend_row0:] = bf16(out[addend_row0:] + addend)."""
     _dev(a), _dev(b)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and a.stride(1) == 1 and b.stride(1) == 1
     M, K = a.shape
@@ -462,9 +466,19 @@ def gemm(a, b, bias=None, epilogue=_lib.MC_EPI_BIAS_BF16, out=None, gate=None, t
     assert out.dtype == want and out.stride(1) == 1 and out.shape == (M, N)
     for v in (bias, gate):
         assert v is None or (v.dtype == torch.float32 and v.is_contiguous())
-    with _Timed(tag, "gemm_other"):
-        check(lib.mc_gemm_bf16(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), M, N, K, bias.data_ptr() if bias is not None else None,
-                               epilogue, out.data_ptr(), out.stride(0), gate.data_ptr() if gate is not None else None, _stream()))
+    bias_p, gate_p = (bias.data_ptr() if bias is not None else None), (gate.data_ptr() if gate is not None else None)
+    if addend is not None:
+        assert epilogue == _lib.MC_EPI_BIAS_GATE_RESID_BF16, "an addend follows the bf16 gated residual only"
+        _dev(addend)
+        assert addend.dtype == torch.bfloat16 and addend.device == out.device and addend.stride(1) == 1
+        assert addend.shape == (M - addend_row0, N), f"addend {tuple(addend.shape)} for rows [{addend_row0}, {M}) x {N} columns"
+        with _Timed(tag, "gemm_other"):
+            check(lib.mc_gemm_bf16_add(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), M, N, K, bias_p, out.data_ptr(), out.stride(0),
+                                       gate_p, addend.data_ptr(), addend.stride(0), addend_row0, _stream()))
+    else:
+        with _Timed(tag, "gemm_other"):
+            check(lib.mc_gemm_bf16(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), M, N, K, bias_p, epilogue, out.data_ptr(),
+                                   out.stride(0), gate_p, _stream()))
     _count()
     return out
 

@@ -377,9 +377,9 @@ class _Sample:
 
 
 def _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance, joint_attention_kwargs,
-                controlnet_block_samples, controlnet_single_block_samples):
-    if joint_attention_kwargs or controlnet_block_samples is not None or controlnet_single_block_samples is not None:
-        raise NotImplementedError("magcache_b200: joint_attention_kwargs / ControlNet residuals are not built for the FLUX engine")
+                controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat):
+    if joint_attention_kwargs:
+        raise NotImplementedError("magcache_b200: joint_attention_kwargs (LoRA scale, ip-adapter) are not built for the FLUX engine")
     if not hidden_states.is_cuda:
         raise RuntimeError("magcache_b200: hidden_states must be CUDA tensors (no CPU path)")
     eng = _cached_engine(self, "_mc_flux_engine", lambda **kw: FluxEngine(FluxWeights.from_module(self, hidden_states.device), **kw))
@@ -388,6 +388,7 @@ def _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, 
     if img_ids.ndim == 3:
         img_ids = img_ids[0]
     eng.stage_inputs(hidden_states, encoder_hidden_states, pooled_projections, timestep, guidance, img_ids, txt_ids)
+    eng.stage_controlnet(controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat)
     return eng
 
 
@@ -396,9 +397,11 @@ def magcache_flux_forward(self, hidden_states, encoder_hidden_states=None, poole
                           controlnet_single_block_samples=None, return_dict=True, controlnet_blocks_repeat=False):
     r"""MagCache4FLUX/magcache_flux.py:234-440 on the H100 kernels: same signature, same state attributes (`cnt, num_steps,
     magcache_thresh, K, retention_ratio, accumulated_ratio / _err / _steps, previous_residual, mag_ratios`), `(output,)` or an object
-    with `.sample`. LoRA scaling, ip-adapter and ControlNet residuals (:275-288, :321-324, :371-381, :410-420) are not built and raise."""
+    with `.sample`. ControlNet residuals (:374-384, :416-423) are added after their blocks on a miss, fused into each block's last GEMM
+    on the image rows; a hit ignores them, as the reference does. LoRA scaling and ip-adapter (:275-288, :321-324) are not built and
+    raise."""
     eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
-                      joint_attention_kwargs, controlnet_block_samples, controlnet_single_block_samples)
+                      joint_attention_kwargs, controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat)
     ctrl = _ctrl(self, "flux")
     skip_forward = ctrl.decide(self)  # :326-338
     _take_residual(eng, self.previous_residual)
@@ -416,9 +419,10 @@ def magcache_flux_calibration(self, hidden_states, encoder_hidden_states=None, p
                               controlnet_single_block_samples=None, return_dict=True, controlnet_blocks_repeat=False):
     r"""MagCache4FLUX/magcache_flux.py:21-231: every call runs the block stack and, from the second call on, records the token-mean
     magnitude ratio, its std and the cosine distance to the previous residual (`norm_ratio / norm_std / cos_dis`, rounded to 5 places);
-    the lists are printed on the last call of a generation and cleared at the wrap (:207-221)."""
+    the lists are printed on the last call of a generation and cleared at the wrap (:207-221). ControlNet residuals as in the
+    forward (:145-155, :187-193); LoRA scaling and ip-adapter raise."""
     eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
-                      joint_attention_kwargs, controlnet_block_samples, controlnet_single_block_samples)
+                      joint_attention_kwargs, controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat)
     if self.cnt == 0:
         eng.res_valid = False  # `if self.cnt>=1` (:199): the first call of a generation has nothing to compare with
     out, stats = eng.calibrate()
