@@ -328,7 +328,8 @@ int32_t mc_gemm_bf16_add(const void* A, int64_t lda, const void* B, int64_t ldb,
  * can be column slices of one fused q|k|v projection buffer; out: [Lq, heads*128] bf16 (ldo). Leading dimensions % 8 == 0,
  * pointers 16-byte aligned.
  * workspace: device scratch for the split-KV partials that small grids use (mc_attn_workspace_bytes tells how much a shape
- * needs; 0 = the shape never splits, workspace may be NULL). The caller owns it: one per stream of concurrent use. */
+ * needs, for every KV tile width a call of that shape may take, whatever MC_ATTN_KERNEL and the key order; 0 = the shape never
+ * splits, workspace may be NULL). The caller owns it: one per stream of concurrent use. */
 int32_t mc_attn_workspace_bytes(int32_t Lq, int32_t Lk, int32_t heads, int64_t* bytes_out);
 int32_t mc_attn_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out,
                     int64_t ldo, int32_t Lq, int32_t Lk, int32_t heads, float scale, void* workspace, int64_t workspace_bytes,

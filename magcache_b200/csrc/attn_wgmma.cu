@@ -8,8 +8,11 @@
 // form (d contiguous, the transposed-B form of wgmma) — the same [rows][64 bf16] 128-byte-swizzled TMA boxes for both, no
 // transposed copy of V anywhere.
 //
-// One kernel, instantiated for two KV tile widths: 128 keys per tile for long key sequences (Lk >= kLongMinLk) and 64 for short
-// ones (text / image cross-attention, refiner). One CTA = one 128-row query tile of one head:
+// One kernel, instantiated for three KV tile widths: 176 keys per tile for long key sequences (Lk >= kLongMinLk), 64 for short
+// ones (text / image cross-attention, refiner), and 128 (MC_ATTN_KERNEL=2, the FMA-pipe exponential variants). The wider the
+// tile, the more keys share each tile's fixed cost (row max, O rescale, fences, barrier turns, mbarrier waits); 176 is the
+// widest whose two-stage K/V ring (2 x 2 x 44 KB + the 32 KB Q tile) fits in shared memory and whose S, P and O fragments fit
+// the consumers' 240 registers without spilling. One CTA = one 128-row query tile of one head:
 //   warpgroup 0     TMA producer (one warp): the Q tile once, then K and V tiles through a two-stage ring
 //   warpgroups 1-2  consumers, 64 query rows each: S = Q K^T (wgmma, both operands in shared memory) into registers, online
 //                   softmax in the exp2 domain on the accumulator fragment (a row spans the 4 lanes of a quad), P rounded to bf16
@@ -18,7 +21,7 @@
 //                   while the tensor cores work on the other's GEMM.
 // The units of a partially filled last wave are split over the KV range and merged by attn_combine_kernel.
 // The 128-key variant can evaluate a fixed fraction of the softmax exponentials on the FMA pipe (ptx::ex2_emul) instead of the
-// MUFU unit; MC_ATTN_EMU selects the fraction per call.
+// MUFU unit; MC_ATTN_EMU selects the fraction per call. The 64- and 176-key variants use the MUFU only.
 #include <cstdlib>
 
 #include "common.cuh"
@@ -120,7 +123,9 @@ struct Layout {
   static constexpr int kVBytes = BKV * kHD * 2;  // two boxes [BKV kv x 64 d]
   static constexpr int kOffK = kQBytes;
   static constexpr int kOffV = kOffK + 2 * kKBytes;
-  static constexpr int kOffBar = kOffV + 2 * kVBytes;  // 160 KB (BKV 128) / 96 KB (BKV 64)
+  static constexpr int kOffBar = kOffV + 2 * kVBytes;  // 208 KB (BKV 176) / 160 KB (BKV 128) / 96 KB (BKV 64)
+  static_assert(kKBytes % 2048 == 0, "every K / V box must start on a 1024-byte swizzle atom");
+  static_assert(kOffBar + 128 <= 227 * 1024, "shared memory per CTA");
   static constexpr int kSmem = kOffBar + 128;
 };
 }  // namespace ak
@@ -233,7 +238,8 @@ __global__ void __launch_bounds__(ak::kThreads, 1)
     // software-pipelined by one tile: S(j) and PV(j-1) are issued back to back, the softmax of tile j runs while PV(j-1) is on
     // the tensor cores, then O is rescaled by f(j) and P(j) packed for the next turn. Every row still sees rescale by f(j),
     // then + P(j) V(j), in tile order, so the result is bit-identical to the serial loop. Live across the wait: O (64 fp32),
-    // S(j) (BKV / 2 fp32) and P(j-1) (BKV / 4 packed bf16x2), ~160 registers for 128-key tiles, within setmaxnreg's 240.
+    // S(j) (BKV / 2 fp32) and P(j-1) (BKV / 4 packed bf16x2): 160 registers for 128-key tiles, 196 for 176-key tiles, within
+    // setmaxnreg's 240.
     //
     // The two consumer warpgroups also take turns: warpgroup w issues its GEMMs only between bar.sync on barrier 1 + w and
     // bar.arrive on the other's barrier 2 - w, so one warpgroup's softmax runs while the tensor cores work through the other's
@@ -259,9 +265,12 @@ __global__ void __launch_bounds__(ak::kThreads, 1)
         // 64-column half (kk >> 2) is a separate TMA box; inside a box one K16 step is 32 B (+2 in the >> 4 field)
         const uint64_t da = ptx::gmma_desc_sw128_kmajor(q_base + (kk >> 2) * (kQBytes / 2)) + 2 * (kk & 3);
         const uint64_t db = ptx::gmma_desc_sw128_kmajor(k_base + s * L::kKBytes + (kk >> 2) * (L::kKBytes / 2)) + 2 * (kk & 3);
-        if constexpr (BKV == 128) {
+        if constexpr (BKV == 176) {
+          ptx::wgmma_m64n176k16_ss(sc, da, db, kk != 0 ? 1u : 0u);
+        } else if constexpr (BKV == 128) {
           ptx::wgmma_m64n128k16_ss(sc, da, db, kk != 0 ? 1u : 0u);
         } else {
+          static_assert(BKV == 64, "KV tile widths: 64, 128, 176");
           ptx::wgmma_m64n64k16_ss(sc, da, db, kk != 0 ? 1u : 0u);
         }
       }
@@ -441,7 +450,6 @@ __global__ void __launch_bounds__(256) attn_combine_kernel(const float* __restri
 
 // ---- host side: work decomposition ----------------------------------------------------------------------------------
 struct AttnPlan {
-  bool long_kernel;
   int q_blocks, kv_tile, total_tiles, rows_per_cta;
   int full_units, tail_units, tail_split;  // see AttnParams
   size_t ws_bytes;                         // workspace for the split partials (0 when nothing is split)
@@ -455,23 +463,35 @@ static int env_int(const char* name, int lo, int hi, int dflt) {
   return (v < lo || v > hi) ? dflt : v;
 }
 
+// KV tile width of a call: 176 keys for long key sequences and for the rotated / flag-gated key order of token-sharded runs, 64
+// for short ones. MC_ATTN_KERNEL forces a width (tests, A-B timing in one process): 1 = 64 keys (not for the rotated /
+// flag-gated order, which keeps 176), 2 = 128 keys (the kernel with the FMA-pipe exponential variants), 3 = 176 keys.
+static int attn_kv_tile(int Lk, bool need_long) {
+  switch (env_int("MC_ATTN_KERNEL", 0, 3, 0)) {
+    case 1: return need_long ? 176 : 64;
+    case 2: return 128;
+    case 3: return 176;
+    default: return (need_long || Lk >= kLongMinLk) ? 176 : 64;
+  }
+}
+
 // One CTA = 128 query rows of one head (one CTA per SM), every unit the same length, so the grid runs in rounds of `slots` CTAs
 // and a partially filled last round costs a whole one (32760 rows x 12 heads = 3072 units on 132 SMs: 23.3 rounds of work take
 // 24; a token-sharded rank's 4095 rows: 384 units, 2.9 rounds take 3). The units
 // of that last round are therefore split over the KV range, floor(slots / units) ways, so that they fill the SMs once at a
-// fraction of the length; a second kernel merges their partial softmaxes. Units of the full rounds are never split.
-static AttnPlan plan_attention(int Lq, int Lk, int heads, bool need_long = false) {
+// fraction of the length; a second kernel merges their partial softmaxes. Units of the full rounds are never split, and no
+// split gets fewer than 512 keys (8 / 4 / 3 tiles of 64 / 128 / 176): below that the pipeline's prologue and epilogue and the
+// merge outweigh the shorter split. At the benchmarked shape: 187 tiles of 176, the 36 units of the last round split 3 ways.
+static AttnPlan plan_attention(int Lq, int Lk, int heads, int kv_tile) {
   AttnPlan pl;
   const int forced_splits = env_int("MC_ATTN_SPLITS", 1, 16, 0);  // MC_ATTN_SPLITS=n: every unit split n ways (1 = never split)
-  const int kernel_sel = env_int("MC_ATTN_KERNEL", 0, 2, 0);  // 0 = by Lk, 1 = 64-key tiles, 2 = 128-key tiles (tests / A-B timing)
-  pl.long_kernel = need_long || kernel_sel == 2 || (kernel_sel == 0 && Lk >= kLongMinLk);  // rotated / flag-gated key order: 128-key tiles
   pl.rows_per_cta = ak::kBQ;
-  pl.kv_tile = pl.long_kernel ? 128 : 64;
+  pl.kv_tile = kv_tile;
   pl.q_blocks = (Lq + pl.rows_per_cta - 1) / pl.rows_per_cta;
   pl.total_tiles = (Lk + pl.kv_tile - 1) / pl.kv_tile;
   const int64_t units = static_cast<int64_t>(pl.q_blocks) * heads;
   const int slots = num_sms();
-  const int min_tiles_per_split = pl.long_kernel ? 4 : 8;
+  const int min_tiles_per_split = (512 + pl.kv_tile - 1) / pl.kv_tile;
   int full = static_cast<int>(units), tail = 0, split = 1;
   if (forced_splits > 0) {
     if (forced_splits > 1) full = 0, tail = static_cast<int>(units), split = forced_splits;
@@ -498,9 +518,14 @@ static AttnPlan plan_attention(int Lq, int Lk, int heads, bool need_long = false
 
 extern "C" int32_t mc_attn_workspace_bytes(int32_t Lq, int32_t Lk, int32_t heads, int64_t* bytes_out) {
   MC_CHECK_ARG(bytes_out != nullptr && Lq >= 1 && Lk >= 1 && heads >= 1, "mc_attn_workspace_bytes: bad arguments");
-  // the larger of the two decompositions the launcher may pick (the rotated / flag-gated form always takes the long kernel)
-  const size_t a = mc::plan_attention(Lq, Lk, heads, false).ws_bytes, b = mc::plan_attention(Lq, Lk, heads, true).ws_bytes;
-  *bytes_out = static_cast<int64_t>(a > b ? a : b);
+  // the largest decomposition over every tile width the launcher may pick, whatever MC_ATTN_KERNEL and the key order, so a
+  // workspace sized once for a shape serves every later call of that shape
+  size_t most = 0;
+  for (const int kv_tile : {64, 128, 176}) {
+    const size_t b = mc::plan_attention(Lq, Lk, heads, kv_tile).ws_bytes;
+    most = b > most ? b : most;
+  }
+  *bytes_out = static_cast<int64_t>(most);
   return MC_OK;
 }
 
@@ -516,7 +541,7 @@ extern "C" int32_t mc_attn_fwd_ex(const void* q, int64_t ldq, const void* k, int
   MC_CHECK_ARG(mc::aligned16(q) && mc::aligned16(k) && mc::aligned16(v) && mc::aligned16(out), "mc_attn_fwd: pointers must be 16-byte aligned");
   MC_CHECK_ARG(first_key_row >= 0 && first_key_row < Lk, "mc_attn_fwd: first_key_row=%d outside [0, %d)", first_key_row, Lk);
   MC_CHECK_ARG(seg_flags == nullptr || (seg_rows >= 1 && seg_epoch != nullptr), "mc_attn_fwd: seg_rows=%d / null epoch", seg_rows);
-  const mc::AttnPlan pl = mc::plan_attention(Lq, Lk, heads, first_key_row != 0 || seg_flags != nullptr);
+  const mc::AttnPlan pl = mc::plan_attention(Lq, Lk, heads, mc::attn_kv_tile(Lk, first_key_row != 0 || seg_flags != nullptr));
   MC_CHECK_ARG(static_cast<int64_t>(pl.q_blocks) * heads * 8 < INT32_MAX, "mc_attn_fwd: grid too large");
   if (pl.tail_units > 0) {
     MC_CHECK_ARG(workspace != nullptr && workspace_bytes >= static_cast<int64_t>(pl.ws_bytes) && (reinterpret_cast<uintptr_t>(workspace) & 31u) == 0,
@@ -548,29 +573,28 @@ extern "C" int32_t mc_attn_fwd_ex(const void* q, int64_t ldq, const void* k, int
 
   dim3 grid(pl.grid(), 1, 1);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (pl.long_kernel) {
-    static mc::PerDeviceOnce once[4];
-    // MC_ATTN_EMU = eighths of the exponentials evaluated on the FMA pipe: 0, 2 (25 %), 3 (37.5 %), 4 (50 %)
-    const int emu = mc::env_int("MC_ATTN_EMU", 0, 4, MC_ATTN_EMU_DEFAULT);
-#define MC_LAUNCH_LONG(MASK, IDX)                                                                                                    \
+  // one PerDeviceOnce per instantiation: [0] 64 keys, [1] 176 keys, [2..5] 128 keys with MC_ATTN_EMU 0 / 2 / 3 / 4
+  static mc::PerDeviceOnce once[6];
+#define MC_LAUNCH(BKV, MASK, IDX)                                                                                                    \
   do {                                                                                                                               \
-    rc = mc::set_max_smem_once(mc::attn_kernel<128, MASK>, mc::ak::Layout<128>::kSmem, once[IDX], "cudaFuncSetAttribute(attn smem)"); \
+    rc = mc::set_max_smem_once(mc::attn_kernel<BKV, MASK>, mc::ak::Layout<BKV>::kSmem, once[IDX], "cudaFuncSetAttribute(attn smem)"); \
     if (rc) return rc;                                                                                                               \
-    mc::attn_kernel<128, MASK><<<grid, mc::ak::kThreads, mc::ak::Layout<128>::kSmem, st>>>(tq, tk, tv, p);                           \
+    mc::attn_kernel<BKV, MASK><<<grid, mc::ak::kThreads, mc::ak::Layout<BKV>::kSmem, st>>>(tq, tk, tv, p);                           \
   } while (0)
-    switch (emu) {
-      case 2: MC_LAUNCH_LONG(0x88u, 1); break;
-      case 3: MC_LAUNCH_LONG(0x92u, 2); break;
-      case 4: MC_LAUNCH_LONG(0xAAu, 3); break;
-      default: MC_LAUNCH_LONG(0x00u, 0); break;
+  if (pl.kv_tile == 176) {
+    MC_LAUNCH(176, 0x00u, 1);
+  } else if (pl.kv_tile == 128) {
+    // MC_ATTN_EMU = eighths of the exponentials evaluated on the FMA pipe: 0, 2 (25 %), 3 (37.5 %), 4 (50 %)
+    switch (mc::env_int("MC_ATTN_EMU", 0, 4, MC_ATTN_EMU_DEFAULT)) {
+      case 2: MC_LAUNCH(128, 0x88u, 3); break;
+      case 3: MC_LAUNCH(128, 0x92u, 4); break;
+      case 4: MC_LAUNCH(128, 0xAAu, 5); break;
+      default: MC_LAUNCH(128, 0x00u, 2); break;
     }
-#undef MC_LAUNCH_LONG
   } else {
-    static mc::PerDeviceOnce once;
-    rc = mc::set_max_smem_once(mc::attn_kernel<64, 0u>, mc::ak::Layout<64>::kSmem, once, "cudaFuncSetAttribute(attn smem)");
-    if (rc) return rc;
-    mc::attn_kernel<64, 0u><<<grid, mc::ak::kThreads, mc::ak::Layout<64>::kSmem, st>>>(tq, tk, tv, p);
+    MC_LAUNCH(64, 0x00u, 0);
   }
+#undef MC_LAUNCH
   MC_CHECK_LAUNCH("attn_kernel launch");
   if (pl.tail_units > 0) {
     const int64_t total = static_cast<int64_t>(pl.tail_units) * pl.rows_per_cta * (mc::kHD / 8);
