@@ -320,6 +320,20 @@ int32_t mc_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, int
 int32_t mc_gemm_bf16_add(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t M, int32_t N, int32_t K,
                          const float* bias, void* out, int64_t ldo, const float* gate, const void* add, int64_t ld_add, int32_t add_row0,
                          void* stream);
+/* An unmerged LoRA update as a second K segment of the same GEMM (PEFT `lora.Linear.forward`: `result = result +
+ * lora_B(lora_A(dropout(x))) * scaling`, run for every adapted Linear of the FLUX forward, MagCache4FLUX/magcache_flux.py:290-430):
+ *   acc[m,n] = sum_k A[m,k] B[n,k] + sum_j U[m,j] T[n,j]           (fp32 accumulation over both segments)
+ * then epilogue `epilogue` (MC_EPI_BIAS_BF16, _GELU_BF16, _GATE_RESID_BF16 or _GATE_RESID_ADD_BF16) on acc exactly as
+ * mc_gemm_bf16 / mc_gemm_bf16_add apply it. U [M, R] is the low-rank activation bf16(x lora_A^T), T [N, R] the scaled rows
+ * bf16(scaling * lora_B). The segment runs as ceil(R / 64) more 64-wide k-blocks of the main loop after the ceil(K / 64) of
+ * (A, B); TMA zero-fills each segment's ragged end, so the sum is that of one plain GEMM over [A | 0 | U | 0] and [B | 0 | T | 0]
+ * with each segment zero-padded to a multiple of 64 columns. R >= 8, R % 8 == 0, ldu / ldt multiples of 8 and >= R, U / T
+ * 16-byte aligned. add / ld_add / add_row0 as in mc_gemm_bf16_add for epilogue 8; add must be NULL for the others.
+ * The rounding chain differs from PEFT's (bf16(bf16(bf16(B bf16(A x)) * s) + bf16(base(x)))): base and update are summed in
+ * fp32 before the epilogue's one rounding. */
+int32_t mc_gemm_bf16_lora(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t M, int32_t N, int32_t K,
+                          const float* bias, int32_t epilogue, void* out, int64_t ldo, const float* gate, const void* add, int64_t ld_add,
+                          int32_t add_row0, const void* U, int64_t ldu, const void* T, int64_t ldt, int32_t R, void* stream);
 
 /* Non-causal attention forward on wgmma: out[i, h*128:(h+1)*128] = softmax(q_h k_h^T * scale) v_h, head_dim = 128
  * (WanSelfAttention / WanT2VCrossAttention [EXT] behind MagCache4Wan2.1/magcache_generate.py:297-298; the joint attention of

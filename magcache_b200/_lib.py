@@ -16,7 +16,7 @@ MC_F32, MC_BF16 = 0, 1
 MC_CMP_LT, MC_CMP_LE = 0, 1
 MC_RETAIN_FLOOR, MC_RETAIN_HALF_UP, MC_RETAIN_CEIL, MC_RETAIN_WAN22_T2V, MC_RETAIN_WAN22_I2V, MC_RETAIN_EXPLICIT = 0, 1, 2, 3, 4, 5
 MC_CTRL_SIGNED_ERR, MC_CTRL_RESET_AT_ZERO, MC_CTRL_RATIO_VETO, MC_CTRL_WRAP_KEEPS_ACC = 1, 2, 4, 8
-ABI_VERSION = 8
+ABI_VERSION = 9
 MC_EPI_BIAS_BF16, MC_EPI_BIAS_GELU_BF16, MC_EPI_BIAS_GATE_RESID, MC_EPI_ROWBIAS_BF16, MC_EPI_BIAS_F32, MC_EPI_BIAS_GELU_ERF_BF16 = 0, 1, 2, 3, 4, 5
 MC_EPI_BIAS_GATE_RESID_BF16, MC_EPI_BIAS_SILU_BF16, MC_EPI_BIAS_GATE_RESID_ADD_BF16 = 6, 7, 8
 
@@ -116,6 +116,8 @@ SIGNATURES = {
                      c_void_p],
     "mc_gemm_bf16_add": [c_void_p, c_int64, c_void_p, c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
                          c_int64, c_int32, c_void_p],
+    "mc_gemm_bf16_lora": [c_void_p, c_int64, c_void_p, c_int64, c_int32, c_int32, c_int32, c_void_p, c_int32, c_void_p, c_int64, c_void_p,
+                          c_void_p, c_int64, c_int32, c_void_p, c_int64, c_void_p, c_int64, c_int32, c_void_p],
     "mc_attn_workspace_bytes": [c_int32, c_int32, c_int32, POINTER(c_int64)],
     "mc_attn_fwd": [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int32, c_int32, c_int32, c_float,
                     c_void_p, c_int64, c_void_p],

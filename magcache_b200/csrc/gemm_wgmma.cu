@@ -62,6 +62,7 @@ struct GemmParams {
   const __nv_bfloat16* add;  // MC_EPI_BIAS_GATE_RESID_ADD_BF16 only: addend rows [add_row0, M), row stride ld_add
   int64_t ld_add;
   int add_row0;
+  int R;  // gemm_bf16_kernel_tail only: width of the second K segment, acc += U[m, :R] . T[n, :R]
 };
 
 // One ROWS-row x 32-column patch: `stage` holds acc[r][c] at stage[r*33 + c]; lane = column. All global accesses below
@@ -218,9 +219,11 @@ __device__ __forceinline__ void epilogue_patch(const GemmParams& p, const float*
   }
 }
 
-template <int EPI, int kBN>
-__global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kGemmThreads, 1)
-    gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
+// The kernel body. kTail: after the ceil(K / 64) k-blocks of (A, B) the same main loop runs ceil(R / 64) more from (U, T), so
+// every epilogue sees acc = A B^T + U T^T (a LoRA update as extra K blocks). Without it tmap_u / tmap_t are never read.
+template <int EPI, int kBN, bool kTail>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap& tmap_u,
+                                          const CUtensorMap& tmap_t, const GemmParams& p) {
   using T = GemmTile<kBN>;
   constexpr int kStageBytes = T::kStageBytes, kOffStaging = T::kOffStaging, kOffBars = T::kOffBars;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -231,6 +234,8 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kGemmThreads,
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = (p.N + kBN - 1) / kBN;
   const int num_kb = (p.K + kBK - 1) / kBK;
+  // k-blocks per tile: TMA zero-fills the ragged ends of both segments, so every stage still carries its full byte count
+  const int total_kb = kTail ? num_kb + (p.R + kBK - 1) / kBK : num_kb;
   // Both CTAs of a cluster walk the same cluster tiles in lock step (the launch makes the grid at most one cluster per tile, so
   // every cluster has at least one step); rank r takes rows [64 r, 64 r + 64) of each, computing on TMA's zero fill where
   // those rows lie past M (the epilogue then writes nothing).
@@ -245,6 +250,10 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kGemmThreads,
     }
     ptx::prefetch_tmap(&tmap_a);
     ptx::prefetch_tmap(&tmap_b);
+    if constexpr (kTail) {
+      ptx::prefetch_tmap(&tmap_u);
+      ptx::prefetch_tmap(&tmap_t);
+    }
     for (int s = 0; s < kStages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
       ptx::mbar_init(&empty_bar[s], kCluster * kEpiWarps);  // one arrival per consumer warp, in each CTA
@@ -264,15 +273,19 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kGemmThreads,
         const int tile = cluster + i * n_clusters;
         const int m0 = (tile / n_tiles) * kClusterBM + static_cast<int>(rank) * kBM, n0 = (tile % n_tiles) * kBN;
         const int nb = n0 + static_cast<int>(rank) * (kBN / kCluster);  // this CTA's half of the B tile
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        for (int kb = 0; kb < total_kb; ++kb, ++it) {
           const int s = it % kStages;
           const uint32_t ph = (it / kStages) & 1;
           ptx::mbar_wait(&empty_bar[s], ph ^ 1);  // released by the consumers of both CTAs: the multicast writes into both
           if (ptx::elect_one()) {
             uint8_t* sa = smem + s * kStageBytes;
+            const bool tail = kTail && kb >= num_kb;
+            const CUtensorMap* ma = tail ? &tmap_u : &tmap_a;
+            const CUtensorMap* mb = tail ? &tmap_t : &tmap_b;
+            const int k0 = (tail ? kb - num_kb : kb) * kBK;
             ptx::mbar_expect_tx(&full_bar[s], kStageBytes);  // own A + both B halves
-            ptx::tma_load_2d(sa, &tmap_a, &full_bar[s], kb * kBK, m0);
-            ptx::tma_load_2d_multicast(sa + kTileABytes + rank * T::kHalfBBytes, &tmap_b, &full_bar[s], kb * kBK, nb,
+            ptx::tma_load_2d(sa, ma, &full_bar[s], k0, m0);
+            ptx::tma_load_2d_multicast(sa + kTileABytes + rank * T::kHalfBBytes, mb, &full_bar[s], k0, nb,
                                        static_cast<uint16_t>((1u << kCluster) - 1));
           }
           __syncwarp();
@@ -290,9 +303,9 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kGemmThreads,
     for (int i = 0; i < steps; ++i) {
       const int tile = cluster + i * n_clusters;
       const int m0 = (tile / n_tiles) * kClusterBM + static_cast<int>(rank) * kBM, n0 = (tile % n_tiles) * kBN;
-      uint32_t it = static_cast<uint32_t>(i) * num_kb;
+      uint32_t it = static_cast<uint32_t>(i) * total_kb;
       int prev_s = -1;
-      for (int kb = 0; kb < num_kb; ++kb, ++it) {
+      for (int kb = 0; kb < total_kb; ++kb, ++it) {
         const int s = it % kStages;
         const uint32_t ph = (it / kStages) & 1;
         ptx::mbar_wait_or_flag(&full_bar[s], ph, timed_out);
@@ -349,10 +362,24 @@ __global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kGemmThreads,
   ptx::cluster_wait();
 }
 
+template <int EPI, int kBN>
+__global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kGemmThreads, 1)
+    gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
+  gemm_body<EPI, kBN, false>(tmap_a, tmap_b, tmap_a, tmap_b, p);
+}
+
+// acc = A B^T + U T^T: tmap_u / tmap_t have the boxes of tmap_a / tmap_b (128 x 64; BN/2 x 64, multicast over the cluster)
+template <int EPI, int kBN>
+__global__ void __cluster_dims__(kCluster, 1, 1) __launch_bounds__(kGemmThreads, 1)
+    gemm_bf16_kernel_tail(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmParams p,
+                          const __grid_constant__ CUtensorMap tmap_u, const __grid_constant__ CUtensorMap tmap_t) {
+  gemm_body<EPI, kBN, true>(tmap_a, tmap_b, tmap_u, tmap_t, p);
+}
+
 // Clusters of this instantiation that fit on the device at once (1 CTA per SM at this shared-memory size), cached per device.
 // Clusters live inside a GPC, so this can be less than SMs / 2; a grid of SMs / 2 clusters would then run a second, nearly
 // empty wave.
-template <int EPI, int BN>
+template <int EPI, int BN, bool kTail>
 static int32_t max_active_clusters(int* out) {
   static int cached[kMaxDevices] = {};
   const int d = current_device();
@@ -365,7 +392,12 @@ static int32_t max_active_clusters(int* out) {
   cfg.blockDim = dim3(kGemmThreads, 1, 1);
   cfg.dynamicSmemBytes = GemmTile<BN>::kSmem;
   int n = 0;
-  const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, gemm_bf16_kernel<EPI, BN>, &cfg);
+  cudaError_t e;
+  if constexpr (kTail) {
+    e = cudaOccupancyMaxActiveClusters(&n, gemm_bf16_kernel_tail<EPI, BN>, &cfg);
+  } else {
+    e = cudaOccupancyMaxActiveClusters(&n, gemm_bf16_kernel<EPI, BN>, &cfg);
+  }
   if (e != cudaSuccess) return cuda_fail(e, "cudaOccupancyMaxActiveClusters(gemm)");
   if (n < 1) {
     set_error("gemm_bf16_kernel: no cluster of %d CTAs with %d B of shared memory fits on this device", kCluster, GemmTile<BN>::kSmem);
@@ -376,20 +408,32 @@ static int32_t max_active_clusters(int* out) {
   return MC_OK;
 }
 
-template <int EPI, int BN>
-static int32_t launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t s) {
+// kTail: gemm_bf16_kernel_tail with tu / tt (non-null), otherwise gemm_bf16_kernel
+template <int EPI, int BN, bool kTail = false>
+static int32_t launch_gemm_bn(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t s, const CUtensorMap* tu = nullptr,
+                              const CUtensorMap* tt = nullptr) {
   static PerDeviceOnce once;
-  int32_t rc = set_max_smem_once(gemm_bf16_kernel<EPI, BN>, GemmTile<BN>::kSmem, once, "cudaFuncSetAttribute(gemm smem)");
+  int32_t rc;
+  if constexpr (kTail) {
+    rc = set_max_smem_once(gemm_bf16_kernel_tail<EPI, BN>, GemmTile<BN>::kSmem, once, "cudaFuncSetAttribute(gemm smem)");
+  } else {
+    rc = set_max_smem_once(gemm_bf16_kernel<EPI, BN>, GemmTile<BN>::kSmem, once, "cudaFuncSetAttribute(gemm smem)");
+  }
   if (rc) return rc;
   int clusters = 0;
-  rc = max_active_clusters<EPI, BN>(&clusters);
+  rc = max_active_clusters<EPI, BN, kTail>(&clusters);
   if (rc) return rc;
   const int m_tiles = (p.M + kClusterBM - 1) / kClusterBM, n_tiles = (p.N + BN - 1) / BN;
   const int total = m_tiles * n_tiles;
   p.total_tiles = total;
   const int grid = kCluster * (total < clusters ? total : clusters);
-  gemm_bf16_kernel<EPI, BN><<<grid, kGemmThreads, GemmTile<BN>::kSmem, s>>>(ta, tb, p);
-  MC_CHECK_LAUNCH("gemm_bf16_kernel launch");
+  if constexpr (kTail) {
+    gemm_bf16_kernel_tail<EPI, BN><<<grid, kGemmThreads, GemmTile<BN>::kSmem, s>>>(ta, tb, p, *tu, *tt);
+    MC_CHECK_LAUNCH("gemm_bf16_kernel_tail launch");
+  } else {
+    gemm_bf16_kernel<EPI, BN><<<grid, kGemmThreads, GemmTile<BN>::kSmem, s>>>(ta, tb, p);
+    MC_CHECK_LAUNCH("gemm_bf16_kernel launch");
+  }
   return MC_OK;
 }
 
@@ -431,7 +475,7 @@ extern "C" int32_t mc_gemm_bf16(const void* A, int64_t lda, const void* B, int64
   int bn = 0;
   const int32_t rc = mc::gemm_prepare("mc_gemm_bf16", A, lda, B, ldb, M, N, K, out, ldo, &ta, &tb, &bn);
   if (rc) return rc;
-  mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0, nullptr, 0, 0};
+  mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0, nullptr, 0, 0, 0};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 #define MC_GEMM_CASE(E) \
   case E: return bn == 128 ? mc::launch_gemm_bn<E, 128>(ta, tb, p, s) : mc::launch_gemm_bn<E, 256>(ta, tb, p, s)
@@ -461,8 +505,50 @@ extern "C" int32_t mc_gemm_bf16_add(const void* A, int64_t lda, const void* B, i
   MC_CHECK_ARG(add, "mc_gemm_bf16_add: null addend");
   MC_CHECK_ARG(ld_add >= N, "mc_gemm_bf16_add: ld_add=%lld < N=%d", static_cast<long long>(ld_add), N);
   MC_CHECK_ARG(add_row0 >= 0 && add_row0 < M, "mc_gemm_bf16_add: add_row0=%d outside [0, M=%d)", add_row0, M);
-  const mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0, static_cast<const __nv_bfloat16*>(add), ld_add, add_row0};
+  const mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0, static_cast<const __nv_bfloat16*>(add), ld_add, add_row0, 0};
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   return bn == 128 ? mc::launch_gemm_bn<MC_EPI_BIAS_GATE_RESID_ADD_BF16, 128>(ta, tb, p, s)
                    : mc::launch_gemm_bn<MC_EPI_BIAS_GATE_RESID_ADD_BF16, 256>(ta, tb, p, s);
+}
+
+extern "C" int32_t mc_gemm_bf16_lora(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t M, int32_t N, int32_t K,
+                                     const float* bias, int32_t epilogue, void* out, int64_t ldo, const float* gate, const void* add,
+                                     int64_t ld_add, int32_t add_row0, const void* U, int64_t ldu, const void* T, int64_t ldt, int32_t R,
+                                     void* stream) {
+  CUtensorMap ta, tb, tu, tt;
+  int bn = 0;
+  int32_t rc = mc::gemm_prepare("mc_gemm_bf16_lora", A, lda, B, ldb, M, N, K, out, ldo, &ta, &tb, &bn);
+  if (rc) return rc;
+  MC_CHECK_ARG(U && T, "mc_gemm_bf16_lora: null U / T");
+  MC_CHECK_ARG(R >= 8 && R % 8 == 0, "mc_gemm_bf16_lora: R=%d must be a positive multiple of 8", R);
+  MC_CHECK_ARG(ldu % 8 == 0 && ldt % 8 == 0 && ldu >= R && ldt >= R, "mc_gemm_bf16_lora: ldu=%lld / ldt=%lld must be multiples of 8 and >= R=%d",
+               static_cast<long long>(ldu), static_cast<long long>(ldt), R);
+  MC_CHECK_ARG(mc::aligned16(U) && mc::aligned16(T), "mc_gemm_bf16_lora: U/T must be 16-byte aligned");
+  if (epilogue == MC_EPI_BIAS_GATE_RESID_ADD_BF16) {
+    MC_CHECK_ARG(add, "mc_gemm_bf16_lora: null addend");
+    MC_CHECK_ARG(ld_add >= N, "mc_gemm_bf16_lora: ld_add=%lld < N=%d", static_cast<long long>(ld_add), N);
+    MC_CHECK_ARG(add_row0 >= 0 && add_row0 < M, "mc_gemm_bf16_lora: add_row0=%d outside [0, M=%d)", add_row0, M);
+  } else {
+    MC_CHECK_ARG(!add, "mc_gemm_bf16_lora: an addend needs epilogue %d", MC_EPI_BIAS_GATE_RESID_ADD_BF16);
+  }
+  rc = mc::make_tmap_bf16_2d(&tu, U, static_cast<uint64_t>(M), static_cast<uint64_t>(R), static_cast<uint64_t>(ldu), mc::kBM, mc::kBK);
+  if (rc) return rc;
+  rc = mc::make_tmap_bf16_2d(&tt, T, static_cast<uint64_t>(N), static_cast<uint64_t>(R), static_cast<uint64_t>(ldt), bn / mc::kCluster, mc::kBK);
+  if (rc) return rc;
+  const mc::GemmParams p{M, N, K, bias, out, ldo, gate, 0, static_cast<const __nv_bfloat16*>(add), ld_add, add_row0, R};
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+#define MC_GEMM_TAIL_CASE(E)                                                            \
+  case E:                                                                               \
+    return bn == 128 ? mc::launch_gemm_bn<E, 128, true>(ta, tb, p, s, &tu, &tt)        \
+                     : mc::launch_gemm_bn<E, 256, true>(ta, tb, p, s, &tu, &tt)
+  switch (epilogue) {
+    MC_GEMM_TAIL_CASE(MC_EPI_BIAS_BF16);
+    MC_GEMM_TAIL_CASE(MC_EPI_BIAS_GELU_BF16);
+    MC_GEMM_TAIL_CASE(MC_EPI_BIAS_GATE_RESID_BF16);
+    MC_GEMM_TAIL_CASE(MC_EPI_BIAS_GATE_RESID_ADD_BF16);
+#undef MC_GEMM_TAIL_CASE
+    default:
+      mc::set_error("mc_gemm_bf16_lora: epilogue %d has no LoRA tail (0, 1, 6 and 8 do)", epilogue);
+      return MC_ERR_INVALID;
+  }
 }

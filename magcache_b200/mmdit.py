@@ -28,6 +28,7 @@ import numpy as np
 import torch
 
 from . import _lib, ops
+from .lora import FluxLoraScan, LoraPack, Tailed, base_linear, is_lora_layer
 
 E = _lib
 
@@ -63,10 +64,13 @@ class Fp8Weight:
 
 
 def linear(a, w, bias, epilogue, out, gate=None, scratch=None, addend=None, addend_row0=0):
-    """`ops.gemm(a, w, ...)` for a bf16 weight (with an `addend`: the ControlNet epilogue, see ops.gemm). For an Fp8Weight: per
+    """`ops.gemm(a, w, ...)` for a bf16 weight (with an `addend`: the ControlNet epilogue, see ops.gemm). A `lora.Tailed` weight adds
+    its LoRA update in the same launch (`ops.gemm(tail=...)`) from the U its group's down-projection left for `a`. For an Fp8Weight: per
     block of rows that fits `scratch` (bf16), one `dequant_fp8_bf16` into the scratch, then the unchanged bf16 GEMM on it for the
     matching output columns. Every epilogue but MC_EPI_ROWBIAS_BF16 is column-wise, so the blocks compute exactly the columns one
     GEMM would."""
+    if isinstance(w, Tailed):
+        return ops.gemm(a, w.w, bias, epilogue, out=out, gate=gate, addend=addend, addend_row0=addend_row0, tail=w.tail(a))
     if not isinstance(w, Fp8Weight):
         if addend is None:
             return ops.gemm(a, w, bias, epilogue, out=out, gate=gate)
@@ -95,20 +99,22 @@ class FluxWeights:
 
     @classmethod
     def from_module(cls, m, dev):
+        """Base weights only: a PEFT LoRA layer contributes its `base_layer`; the adapters are read at every call (lora.py)."""
         cfg = m.config
         w = cls()
+        B = base_linear
         w.heads, w.head_dim = cfg.num_attention_heads, cfg.attention_head_dim
         if w.head_dim != 128 or tuple(cfg.axes_dims_rope) != (16, 56, 56):
             raise NotImplementedError("FLUX engine: head_dim 128 with RoPE axes (16, 56, 56)")
         w.dim = D = w.heads * w.head_dim
         w.in_channels, w.joint_dim, w.pooled_dim = cfg.in_channels, cfg.joint_attention_dim, cfg.pooled_projection_dim
         w.guidance = bool(cfg.guidance_embeds)
-        w.x_w, w.x_b = _w(m.x_embedder.weight, dev), _b(m.x_embedder.bias, dev)
-        w.ctx_w, w.ctx_b = _w(m.context_embedder.weight, dev), _b(m.context_embedder.bias, dev)
+        w.x_w, w.x_b = _w(B(m.x_embedder).weight, dev), _b(B(m.x_embedder).bias, dev)
+        w.ctx_w, w.ctx_b = _w(B(m.context_embedder).weight, dev), _b(B(m.context_embedder).bias, dev)
         tte = m.time_text_embed
 
         def mlp(e):
-            return (_w(e.linear_1.weight, dev), _b(e.linear_1.bias, dev), _w(e.linear_2.weight, dev), _b(e.linear_2.bias, dev))
+            return (_w(B(e.linear_1).weight, dev), _b(B(e.linear_1).bias, dev), _w(B(e.linear_2).weight, dev), _b(B(e.linear_2).bias, dev))
 
         w.t_mlp, w.p_mlp = mlp(tte.timestep_embedder), mlp(tte.text_embedder)
         w.g_mlp = mlp(tte.guidance_embedder) if w.guidance else None
@@ -116,40 +122,40 @@ class FluxWeights:
 
         def ada(lin):
             nonlocal off
-            ada_w.append(lin.weight.detach())
-            ada_b.append(lin.bias.detach())
-            start, off = off, off + lin.weight.shape[0]
+            ada_w.append(B(lin).weight.detach())
+            ada_b.append(B(lin).bias.detach())
+            start, off = off, off + B(lin).weight.shape[0]
             return start
 
         for blk in m.transformer_blocks:
             a = blk.attn
             w.double.append({
                 "ada": ada(blk.norm1.linear), "ada_c": ada(blk.norm1_context.linear),
-                "qk_w": _w(torch.cat([a.to_q.weight, a.to_k.weight], 0), dev), "qk_b": _b(torch.cat([a.to_q.bias, a.to_k.bias], 0), dev),
-                "v_w": _w(a.to_v.weight, dev), "v_b": _b(a.to_v.bias, dev), "o_w": _w(a.to_out[0].weight, dev), "o_b": _b(a.to_out[0].bias, dev),
+                "qk_w": _w(torch.cat([B(a.to_q).weight, B(a.to_k).weight], 0), dev), "qk_b": _b(torch.cat([B(a.to_q).bias, B(a.to_k).bias], 0), dev),
+                "v_w": _w(B(a.to_v).weight, dev), "v_b": _b(B(a.to_v).bias, dev), "o_w": _w(B(a.to_out[0]).weight, dev), "o_b": _b(B(a.to_out[0]).bias, dev),
                 "nq": _b(a.norm_q.weight, dev), "nk": _b(a.norm_k.weight, dev),
-                "cqk_w": _w(torch.cat([a.add_q_proj.weight, a.add_k_proj.weight], 0), dev),
-                "cqk_b": _b(torch.cat([a.add_q_proj.bias, a.add_k_proj.bias], 0), dev),
-                "cv_w": _w(a.add_v_proj.weight, dev), "cv_b": _b(a.add_v_proj.bias, dev),
-                "co_w": _w(a.to_add_out.weight, dev), "co_b": _b(a.to_add_out.bias, dev),
+                "cqk_w": _w(torch.cat([B(a.add_q_proj).weight, B(a.add_k_proj).weight], 0), dev),
+                "cqk_b": _b(torch.cat([B(a.add_q_proj).bias, B(a.add_k_proj).bias], 0), dev),
+                "cv_w": _w(B(a.add_v_proj).weight, dev), "cv_b": _b(B(a.add_v_proj).bias, dev),
+                "co_w": _w(B(a.to_add_out).weight, dev), "co_b": _b(B(a.to_add_out).bias, dev),
                 "cnq": _b(a.norm_added_q.weight, dev), "cnk": _b(a.norm_added_k.weight, dev),
-                "ff1_w": _w(blk.ff.net[0].proj.weight, dev), "ff1_b": _b(blk.ff.net[0].proj.bias, dev),
-                "ff2_w": _w(blk.ff.net[2].weight, dev), "ff2_b": _b(blk.ff.net[2].bias, dev),
-                "cff1_w": _w(blk.ff_context.net[0].proj.weight, dev), "cff1_b": _b(blk.ff_context.net[0].proj.bias, dev),
-                "cff2_w": _w(blk.ff_context.net[2].weight, dev), "cff2_b": _b(blk.ff_context.net[2].bias, dev),
+                "ff1_w": _w(B(blk.ff.net[0].proj).weight, dev), "ff1_b": _b(B(blk.ff.net[0].proj).bias, dev),
+                "ff2_w": _w(B(blk.ff.net[2]).weight, dev), "ff2_b": _b(B(blk.ff.net[2]).bias, dev),
+                "cff1_w": _w(B(blk.ff_context.net[0].proj).weight, dev), "cff1_b": _b(B(blk.ff_context.net[0].proj).bias, dev),
+                "cff2_w": _w(B(blk.ff_context.net[2]).weight, dev), "cff2_b": _b(B(blk.ff_context.net[2]).bias, dev),
             })
         for blk in m.single_transformer_blocks:
             a = blk.attn
             w.single.append({
                 "ada": ada(blk.norm.linear),
-                "qk_w": _w(torch.cat([a.to_q.weight, a.to_k.weight], 0), dev), "qk_b": _b(torch.cat([a.to_q.bias, a.to_k.bias], 0), dev),
-                "v_w": _w(a.to_v.weight, dev), "v_b": _b(a.to_v.bias, dev), "nq": _b(a.norm_q.weight, dev), "nk": _b(a.norm_k.weight, dev),
-                "mlp_w": _w(blk.proj_mlp.weight, dev), "mlp_b": _b(blk.proj_mlp.bias, dev),
-                "out_w": _w(blk.proj_out.weight, dev), "out_b": _b(blk.proj_out.bias, dev),
+                "qk_w": _w(torch.cat([B(a.to_q).weight, B(a.to_k).weight], 0), dev), "qk_b": _b(torch.cat([B(a.to_q).bias, B(a.to_k).bias], 0), dev),
+                "v_w": _w(B(a.to_v).weight, dev), "v_b": _b(B(a.to_v).bias, dev), "nq": _b(a.norm_q.weight, dev), "nk": _b(a.norm_k.weight, dev),
+                "mlp_w": _w(B(blk.proj_mlp).weight, dev), "mlp_b": _b(B(blk.proj_mlp).bias, dev),
+                "out_w": _w(B(blk.proj_out).weight, dev), "out_b": _b(B(blk.proj_out).bias, dev),
             })
         w.ada_out = ada(m.norm_out.linear)
         w.ada_w, w.ada_b, w.ada_rows = _w(torch.cat(ada_w, 0), dev), _b(torch.cat(ada_b, 0), dev), off
-        w.out_w, w.out_b = _w(m.proj_out.weight, dev), _b(m.proj_out.bias, dev)
+        w.out_w, w.out_b = _w(B(m.proj_out).weight, dev), _b(B(m.proj_out).bias, dev)
         w.device = dev
         return w
 
@@ -176,6 +182,7 @@ class MMDiTCore:
     ada_w / ada_b / ada_rows), the token order (`txt_first`), the RoPE table of the rows that get RoPE, and its own prologue / head."""
 
     txt_first = True
+    lora = None  # lora.LoraPack of the current call (FLUX with unmerged adapters), else None
 
     def _controlnet_views(self):
         """`run_blocks`' ControlNet argument for the current call; only the FLUX engine takes ControlNet residuals."""
@@ -230,11 +237,13 @@ class MMDiTCore:
         """Every `Linear(silu(vec))` of the block stack (AdaLayerNormZero / ModulateDiT / final layer) from ONE GEMM: they depend on the
         conditioning vector only. bf16 like the reference, then an exact fp32 copy for the kernels that read modulation / gates."""
         w = self.w
-        if w.ada_parts is None:
+        parts = w.ada_parts if self.lora is None or self.lora.ada_parts is None else self.lora.ada_parts
+        if parts is None:
             ops.gemm(ops.silu(vec), w.ada_w, w.ada_b, E.MC_EPI_BIAS_BF16, out=self.ada)
-        else:  # FP8 block rows and bf16 final-layer rows: each output column still comes from its own row of the stack
-            s = ops.silu(vec)
-            for r0, wt in w.ada_parts:
+        else:  # FP8 block rows and bf16 final-layer rows, or LoRA-adapted rows apart from the others: each output column still
+            s = ops.silu(vec)  # comes from its own row of the stack
+            self._down(self.lora.groups if self.lora is not None else {}, "ada", s)
+            for r0, wt in parts:
                 r1 = r0 + wt.shape[0]
                 self._linear(s, wt, w.ada_b[r0:r1], E.MC_EPI_BIAS_BF16, out=self.ada[:, r0:r1])
         ops.cast_into(self.ada.view(-1), self.adaf)
@@ -246,6 +255,13 @@ class MMDiTCore:
     def _rope_for(self, rows):
         """RoPE table rows for a token range, or None when that range gets no RoPE (HunyuanVideo text tokens)."""
         raise NotImplementedError
+
+    @staticmethod
+    def _down(groups, key, x):
+        """The LoRA down-projection U = bf16(x A^T) of the adapters that read the GEMM input `x` (plain GEMM, no bias), if any."""
+        g = groups.get(key)
+        if g is not None:
+            g.u, g.src = ops.gemm(x, g.A), x
 
     # ------------------------------------------------------------------------------------------ attention over the joint sequence
     def _project(self, rows, h_rows, qk_w, qk_b, v_w, v_b):
@@ -316,35 +332,47 @@ class MMDiTCore:
         fused into the block's last GEMM on the image rows (MC_EPI_BIAS_GATE_RESID_ADD_BF16): FF2 of the image stream of a double
         block, the `out` GEMM of a single block from row n_txt on (text rows first, FLUX only)."""
         w, D, S = self.w, self.w.dim, self.S
+        double, single = (w.double, w.single) if self.lora is None else (self.lora.double, self.lora.single)
         c_double, c_single = ctrl if ctrl is not None else ((None,) * len(w.double), (None,) * len(w.single))
         txt, img = self.txt, self.img
         hs, h = self.hs, self.h
-        for b, add in zip(w.double, c_double):
+        down = self._down
+        for b, add in zip(double, c_double):
+            lg = b.get("lora", {})  # this block's LoRA down-projections, keyed by the GEMM input they read
             em, emc = self._em(b["ada"], 6), self._em(b["ada_c"], 6)  # (shift1, scale1, gate1, shift2, scale2, gate2)
             ops.ln_modulate(hs[img], em, 1, 0, round_ln_to_bf16=True, out=h[img])
             ops.ln_modulate(hs[txt], emc, 1, 0, round_ln_to_bf16=True, out=h[txt])
+            down(lg, "h", h[img])
+            down(lg, "ch", h[txt])
             self._project(img, h[img], b["qk_w"], b["qk_b"], b["v_w"], b["v_b"])
             self._project(txt, h[txt], b["cqk_w"], b["cqk_b"], b["cv_w"], b["cv_b"])
             self._qk_norm(img, b["nq"], b["nk"])
             self._qk_norm(txt, b["cnq"], b["cnk"])
             self._joint_attention(self.att)
+            down(lg, "att", self.att[img])
+            down(lg, "catt", self.att[txt])
             self._linear(self.att[img], b["o_w"], b["o_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[img], gate=em[2])
             self._linear(self.att[txt], b["co_w"], b["co_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[txt], gate=emc[2])
-            for rows, e, f1w, f1b, f2w, f2b in ((img, em, b["ff1_w"], b["ff1_b"], b["ff2_w"], b["ff2_b"]),
-                                                (txt, emc, b["cff1_w"], b["cff1_b"], b["cff2_w"], b["cff2_b"])):
+            for rows, e, f1w, f1b, f2w, f2b, pre in ((img, em, b["ff1_w"], b["ff1_b"], b["ff2_w"], b["ff2_b"], ""),
+                                                     (txt, emc, b["cff1_w"], b["cff1_b"], b["cff2_w"], b["cff2_b"], "c")):
                 ops.ln_modulate(hs[rows], e, 4, 3, round_ln_to_bf16=True, out=h[rows])
+                down(lg, pre + "h2", h[rows])
                 ffh = self.cat[rows][:, D:]
                 self._linear(h[rows], f1w, f1b, E.MC_EPI_BIAS_GELU_BF16, out=ffh)
+                down(lg, pre + "ffh", ffh)
                 self._linear(ffh, f2w, f2b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[rows], gate=e[5], addend=add if rows == img else None)
         allr = slice(0, S)
-        for b, add in zip(w.single, c_single):
+        for b, add in zip(single, c_single):
+            lg = b.get("lora", {})
             em = self._em(b["ada"], 3)  # (shift, scale, gate)
             ops.ln_modulate(hs, em, 1, 0, round_ln_to_bf16=True, out=h)
+            down(lg, "h", h)
             self._linear(h, b["mlp_w"], b["mlp_b"], E.MC_EPI_BIAS_GELU_BF16, out=self.cat[:, D:])
             self._project(allr, h, b["qk_w"], b["qk_b"], b["v_w"], b["v_b"])
             self._qk_norm(img, b["nq"], b["nk"])
             self._qk_norm(txt, b["nq"], b["nk"])
             self._joint_attention(self.cat[:, :D])
+            down(lg, "cat", self.cat)
             self._linear(self.cat, b["out_w"], b["out_b"], E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs, gate=em[2], addend=add,
                          addend_row0=self.n_txt)
         return hs[img]
@@ -406,6 +434,25 @@ class FluxEngine(MMDiTCore):
         self._rope_key, self._rope = None, None
         self.res_valid = False
         self.controlnet = (None, None, False)
+        self._lora_scan, self._lora_merged, self._lora_wrappers = None, (), ()
+
+    def sync_lora(self, module):
+        """Take the module's unmerged LoRA adapters as they are now (lora.FluxLoraScan): called at every forward, after the
+        reference's `scale_lora_layers`. Base weights are repacked from the module when a merge or unmerge happened since they
+        were packed, and when a LoRA layer seen before has left the module (it may have been merged first: `fuse_lora()` then
+        `unload_lora_weights()`); otherwise only what changed is repacked (lora.LoraPack)."""
+        first = self._lora_scan is None
+        if first:
+            self._lora_scan = FluxLoraScan(module)
+        spec, merged, wrappers, changed = self._lora_scan.scan()
+        now = {id(m) for m in wrappers}
+        if not first and (merged != self._lora_merged or any(id(m) not in now for m in self._lora_wrappers)):
+            self.w = FluxWeights.from_module(module, self.device)
+            self.lora, changed = None, True
+        # the layers themselves are kept (not their ids), so an id cannot be reused by a new layer before the next comparison
+        self._lora_merged, self._lora_wrappers = merged, wrappers
+        if changed:
+            self.lora = LoraPack(self.w, spec, self.lora) if spec else None
 
     def _workspace(self, n_img, n_txt):
         if self._shape == (n_img, n_txt):
@@ -484,13 +531,16 @@ class FluxEngine(MMDiTCore):
     def prologue(self):
         """x_embedder, time_text_embed, context_embedder (:290-303) and every AdaLayerNorm projection of the forward."""
         w = self.w
-        ops.gemm(self.s_hidden, w.x_w, w.x_b, E.MC_EPI_BIAS_BF16, out=self.x0)
+        top, lg = (self.lora.top, self.lora.groups) if self.lora is not None else ({"x_w": w.x_w, "ctx_w": w.ctx_w}, {})
+        self._down(lg, "x", self.s_hidden)
+        self._linear(self.s_hidden, top["x_w"], w.x_b, E.MC_EPI_BIAS_BF16, out=self.x0)
         temb = self._time_mlp(self._sinusoid(self.s_t[0:1]), w.t_mlp)
         if w.guidance:
             temb = ops.cache_hit_add(temb, self._time_mlp(self._sinusoid(self.s_t[1:2]), w.g_mlp))
         temb = ops.cache_hit_add(temb, self._time_mlp(self.s_pooled, w.p_mlp))
         self._modulation_table(temb)
-        ops.gemm(self.s_enc, w.ctx_w, w.ctx_b, E.MC_EPI_BIAS_BF16, out=self.hs[self.txt])
+        self._down(lg, "ctx", self.s_enc)
+        self._linear(self.s_enc, top["ctx_w"], w.ctx_b, E.MC_EPI_BIAS_BF16, out=self.hs[self.txt])
         return self.x0
 
     def head(self, x_img):
@@ -498,7 +548,10 @@ class FluxEngine(MMDiTCore):
         w = self.w
         em = self._em(w.ada_out, 2)
         ops.ln_modulate(x_img, em, 0, 1, round_ln_to_bf16=True, out=self.h[self.img])
-        return self._gather_output(ops.gemm(self.h[self.img], w.out_w, w.out_b, E.MC_EPI_BIAS_BF16))
+        if self.lora is None:
+            return self._gather_output(ops.gemm(self.h[self.img], w.out_w, w.out_b, E.MC_EPI_BIAS_BF16))
+        self._down(self.lora.groups, "head", self.h[self.img])
+        return self._gather_output(self._linear(self.h[self.img], self.lora.top["out_w"], w.out_b, E.MC_EPI_BIAS_BF16, out=None))
 
 
 # ======================================================================================================================
@@ -548,6 +601,10 @@ class HunyuanWeights:
 
     @classmethod
     def from_module(cls, m, dev):
+        for name, mod in m.named_modules():  # HunyuanVideo's reference forward has no LoRA path
+            if is_lora_layer(mod):
+                raise NotImplementedError(f"magcache_b200: the HunyuanVideo engine runs no LoRA adapters; {name} carries one "
+                                          "(merge it into the weights first)")
         w = cls()
         w.dim = D = m.hidden_size
         w.heads = m.heads_num

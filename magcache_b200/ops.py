@@ -448,12 +448,15 @@ def silu(x, out=None):
     return out
 
 
-def gemm(a, b, bias=None, epilogue=_lib.MC_EPI_BIAS_BF16, out=None, gate=None, tag=None, addend=None, addend_row0=0):
+def gemm(a, b, bias=None, epilogue=_lib.MC_EPI_BIAS_BF16, out=None, gate=None, tag=None, addend=None, addend_row0=0, tail=None):
     """acc = a @ b.T on wgmma (a [M,K] bf16, b [N,K] bf16, row stride allowed) + fused epilogue (see MC_EPI_*).
 
     `addend` (bf16 [M - addend_row0, N], unit column stride, row stride allowed) turns MC_EPI_BIAS_GATE_RESID_BF16 into
     MC_EPI_BIAS_GATE_RESID_ADD_BF16 (`mc_gemm_bf16_add`): epilogue 6 in place on `out`, then
-    out[addend_row0:] = bf16(out[addend_row0:] + addend)."""
+    out[addend_row0:] = bf16(out[addend_row0:] + addend).
+
+    `tail` = (U [M, R], T [N, R]) bf16, R a multiple of 8: acc += U @ T.T as more k-blocks of the same main loop
+    (`mc_gemm_bf16_lora`, a LoRA update), for MC_EPI_BIAS_BF16, _GELU_BF16, _GATE_RESID_BF16 and, with an addend, _GATE_RESID_ADD_BF16."""
     _dev(a), _dev(b)
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16 and a.stride(1) == 1 and b.stride(1) == 1
     M, K = a.shape
@@ -472,6 +475,19 @@ def gemm(a, b, bias=None, epilogue=_lib.MC_EPI_BIAS_BF16, out=None, gate=None, t
         _dev(addend)
         assert addend.dtype == torch.bfloat16 and addend.device == out.device and addend.stride(1) == 1
         assert addend.shape == (M - addend_row0, N), f"addend {tuple(addend.shape)} for rows [{addend_row0}, {M}) x {N} columns"
+    if tail is not None:
+        u, t = tail
+        _dev(u), _dev(t)
+        R = u.shape[1]
+        assert u.dtype == torch.bfloat16 and t.dtype == torch.bfloat16 and u.stride(1) == 1 and t.stride(1) == 1
+        assert u.shape == (M, R) and t.shape == (N, R), f"tail U {tuple(u.shape)} / T {tuple(t.shape)} for M={M} N={N}"
+        epi = _lib.MC_EPI_BIAS_GATE_RESID_ADD_BF16 if addend is not None else epilogue
+        with _Timed(tag, "gemm_other"):
+            check(lib.mc_gemm_bf16_lora(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), M, N, K, bias_p, epi, out.data_ptr(),
+                                        out.stride(0), gate_p, addend.data_ptr() if addend is not None else None,
+                                        addend.stride(0) if addend is not None else 0, addend_row0, u.data_ptr(), u.stride(0),
+                                        t.data_ptr(), t.stride(0), R, _stream()))
+    elif addend is not None:
         with _Timed(tag, "gemm_other"):
             check(lib.mc_gemm_bf16_add(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), M, N, K, bias_p, out.data_ptr(), out.stride(0),
                                        gate_p, addend.data_ptr(), addend.stride(0), addend_row0, _stream()))

@@ -12,6 +12,7 @@ accumulated_steps, residual_cache, mag_ratios`; calibration: `norm_ratio, norm_s
 reference. Everything between the Python call and the returned tensors runs on the CUDA kernels of libmagcache_b200.so;
 there is no eager/PyTorch fallback — a CPU tensor or a missing library raises.
 """
+import contextlib
 import os
 
 import numpy as np
@@ -21,6 +22,7 @@ import torch
 from . import ops
 from .config import FAMILIES, interp_cfg, nearest_interp, save_json, table_for_ckpt_dir, table_from_calibration, tables
 from .controller import AttrController, OpenSoraTeaController, TeaController, opensora_rel_l1
+from .lora import is_lora_layer, scale_lora_layers, unscale_lora_layers
 from .mmdit import FluxEngine, FluxWeights, HunyuanEngine, HunyuanWeights
 from .opensora import OpenSoraEngine, OpenSoraWeights
 from .wan import WanEngine, WanWeights
@@ -42,7 +44,8 @@ def _cached_engine(self, attr, build):
 def invalidate_engine(model):
     """Drop the engine cached on `model` (and with it the repacked bf16 copy of the weights, the workspaces and any captured CUDA
     graphs) and its controllers. The engine snapshots the module's parameters at the first forward: call this after anything that
-    changes them — a LoRA merge, `load_state_dict`, `.to(...)` — and the next forward repacks. The module's own parameters stay
+    changes them — a LoRA merge (on a FLUX model only one whose LoRA layers are then removed before the next forward, see
+    lora.FluxLoraScan), `load_state_dict`, `.to(...)` — and the next forward repacks. The module's own parameters stay
     resident next to the packed copy (about +2.8 GB for the 1.3B model, +28 GB for 14B); free or offload them yourself if that matters."""
     for name in ENGINE_ATTRS + ("_mc_ctrls",):
         model.__dict__.pop(name, None)
@@ -376,13 +379,40 @@ class _Sample:
         self.sample = sample
 
 
-def _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance, joint_attention_kwargs,
-                controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat):
-    if joint_attention_kwargs:
-        raise NotImplementedError("magcache_b200: joint_attention_kwargs (LoRA scale, ip-adapter) are not built for the FLUX engine")
+def _flux_lora_scale(self, hidden_states, joint_attention_kwargs):
+    """The call's LoRA scale (:274-279), after the checks that need no engine: only a "scale" key is built, CUDA inputs only."""
+    extra = sorted(k for k in (joint_attention_kwargs or {}) if k != "scale")
+    if extra:
+        raise NotImplementedError(f"magcache_b200: joint_attention_kwargs {extra} (ip-adapter, ...) are not built for the FLUX engine; "
+                                  "only the LoRA 'scale' is")
     if not hidden_states.is_cuda:
         raise RuntimeError("magcache_b200: hidden_states must be CUDA tensors (no CPU path)")
+    lora_scale = joint_attention_kwargs.get("scale", 1.0) if joint_attention_kwargs is not None else 1.0
+    if lora_scale != 1.0 and not (isinstance(self, torch.nn.Module) and any(is_lora_layer(m) for m in self.modules())):
+        # the reference would scale nothing: a scale without adapters is taken for adapters that failed to load
+        raise NotImplementedError(f"magcache_b200: joint_attention_kwargs scale={lora_scale} but the model has no LoRA layer to scale")
+    return lora_scale
+
+
+@contextlib.contextmanager
+def _lora_scaled(self, lora_scale):
+    """The reference's `scale_lora_layers` before the forward (:281-283) and `unscale_lora_layers` after it (:437-439). The unscale
+    also runs when the engine refuses an input mid-call (an unsupported adapter, a malformed ControlNet sample), so a caller that
+    catches the error never finds the layers' `scaling` left multiplied by the scale."""
+    scale_lora_layers(self, lora_scale)
+    try:
+        yield
+    finally:
+        unscale_lora_layers(self, lora_scale)
+
+
+def _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
+                controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat):
+    """Stages one FLUX call on the engine (inside `_lora_scaled`) and hands it the adapters as they are now."""
+    is_module = isinstance(self, torch.nn.Module)
     eng = _cached_engine(self, "_mc_flux_engine", lambda **kw: FluxEngine(FluxWeights.from_module(self, hidden_states.device), **kw))
+    if is_module:  # (a benchmark's MMDiTHandle sets the engine's LoRA pack itself)
+        eng.sync_lora(self)
     if txt_ids.ndim == 3:  # :305-316 (deprecated 3-D ids)
         txt_ids = txt_ids[0]
     if img_ids.ndim == 3:
@@ -398,16 +428,19 @@ def magcache_flux_forward(self, hidden_states, encoder_hidden_states=None, poole
     r"""MagCache4FLUX/magcache_flux.py:234-440 on the H100 kernels: same signature, same state attributes (`cnt, num_steps,
     magcache_thresh, K, retention_ratio, accumulated_ratio / _err / _steps, previous_residual, mag_ratios`), `(output,)` or an object
     with `.sample`. ControlNet residuals (:374-384, :416-423) are added after their blocks on a miss, fused into each block's last GEMM
-    on the image rows; a hit ignores them, as the reference does. LoRA scaling and ip-adapter (:275-288, :321-324) are not built and
-    raise."""
-    eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
-                      joint_attention_kwargs, controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat)
-    ctrl = _ctrl(self, "flux")
-    skip_forward = ctrl.decide(self)  # :326-338
-    _take_residual(eng, self.previous_residual)
-    out = eng.forward("hit" if skip_forward else "miss")
-    self.previous_residual = eng.res.view(1, *eng.res.shape)  # :427
-    ctrl.advance(self)  # :431-436
+    on the image rows; a hit ignores them, as the reference does. Unmerged PEFT LoRA adapters run as tails of the GEMMs of the
+    Linears they adapt (magcache_b200/lora.py), scaled by `joint_attention_kwargs["scale"]` with the reference's
+    scale / unscale statements (:274-287, :437-439) on every call, hit or miss. ip-adapter (:321-324) is not built and raises."""
+    lora_scale = _flux_lora_scale(self, hidden_states, joint_attention_kwargs)
+    with _lora_scaled(self, lora_scale):
+        eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
+                          controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat)
+        ctrl = _ctrl(self, "flux")
+        skip_forward = ctrl.decide(self)  # :326-338
+        _take_residual(eng, self.previous_residual)
+        out = eng.forward("hit" if skip_forward else "miss")
+        self.previous_residual = eng.res.view(1, *eng.res.shape)  # :427
+        ctrl.advance(self)  # :431-436
     output = out.view(1, *out.shape)
     if not return_dict:
         return (output,)
@@ -420,21 +453,23 @@ def magcache_flux_calibration(self, hidden_states, encoder_hidden_states=None, p
     r"""MagCache4FLUX/magcache_flux.py:21-231: every call runs the block stack and, from the second call on, records the token-mean
     magnitude ratio, its std and the cosine distance to the previous residual (`norm_ratio / norm_std / cos_dis`, rounded to 5 places);
     the lists are printed on the last call of a generation and cleared at the wrap (:207-221). ControlNet residuals as in the
-    forward (:145-155, :187-193); LoRA scaling and ip-adapter raise."""
-    eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
-                      joint_attention_kwargs, controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat)
-    if self.cnt == 0:
-        eng.res_valid = False  # `if self.cnt>=1` (:199): the first call of a generation has nothing to compare with
-    out, stats = eng.calibrate()
-    if stats is not None:
-        _record_stats(self, stats)
-    self.previous_residual = eng.res.view(1, *eng.res.shape)
-    if self.cnt >= self.num_steps - 1:
-        _print_stats(self)
-    self.cnt += 1
-    if self.cnt >= self.num_steps:
-        self.cnt = 0
-        self.norm_ratio, self.norm_std, self.cos_dis = [], [], []
+    forward (:145-155, :187-193); LoRA adapters and scale as in the forward (:62-75, :224-226); ip-adapter raises."""
+    lora_scale = _flux_lora_scale(self, hidden_states, joint_attention_kwargs)
+    with _lora_scaled(self, lora_scale):
+        eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
+                          controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat)
+        if self.cnt == 0:
+            eng.res_valid = False  # `if self.cnt>=1` (:199): the first call of a generation has nothing to compare with
+        out, stats = eng.calibrate()
+        if stats is not None:
+            _record_stats(self, stats)
+        self.previous_residual = eng.res.view(1, *eng.res.shape)
+        if self.cnt >= self.num_steps - 1:
+            _print_stats(self)
+        self.cnt += 1
+        if self.cnt >= self.num_steps:
+            self.cnt = 0
+            self.norm_ratio, self.norm_std, self.cos_dis = [], [], []
     output = out.view(1, *out.shape)
     return _Sample(output) if return_dict else (output,)
 

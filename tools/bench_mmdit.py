@@ -4,10 +4,15 @@ Not the contract bench (bench.py measures the north-star Wan2.1 workload); writt
 
 usage (GPU): python tools/bench_mmdit.py flux|hunyuan [--steps N] [--no-cache] [--tokens-scale F]
              python tools/bench_mmdit.py flux --controlnet D,S [--controlnet-repeat] [--rounds R] [--steps N]
+             python tools/bench_mmdit.py flux --lora RANK [--rounds R] [--steps N]
 
 --controlnet D,S: the FLUX 1024^2 miss forward (the whole block stack) with D double-block and S single-block synthetic bf16
 ControlNet samples (S = 0: none for the single blocks) against the same forward without samples, timed in alternating rounds of N
-forwards each with CUDA events; prints the card name and power limit beside the times."""
+forwards each with CUDA events; prints the card name and power limit beside the times.
+
+--lora RANK: the FLUX 1024^2 miss and hit forwards with one synthetic rank-RANK LoRA adapter on every covered target (every block
+Linear, every AdaLayerNorm projection, x_embedder, context_embedder, proj_out; magcache_b200/lora.py) against the same forwards
+without adapters, alternating rounds as for --controlnet."""
 import argparse
 import json
 import os
@@ -33,9 +38,8 @@ def card():
     return name.strip() or torch.cuda.get_device_name(0), power.strip() or "unknown"
 
 
-def bench_controlnet(n_double, n_single, repeat, rounds, per_round):
-    """Miss forwards at the FLUX.1-dev 1024^2 shape (4096 image + 512 text tokens), without and with ControlNet samples,
-    alternating; the two outputs differ only through the samples."""
+def _flux_1024_engine():
+    """A FLUX.1-dev engine on synthetic weights, staged at 1024^2 (4096 image + 512 text tokens)."""
     dev = torch.device("cuda:0")
     g = torch.Generator(device=dev).manual_seed(0)
     eng = mmdit.FluxEngine(mmdit.random_flux_weights(dev))
@@ -45,27 +49,43 @@ def bench_controlnet(n_double, n_single, repeat, rounds, per_round):
     eng.stage_inputs(torch.randn(1, n_img, 64, device=dev, generator=g).bfloat16(), torch.randn(1, n_txt, 4096, device=dev, generator=g).bfloat16(),
                      torch.randn(1, 768, device=dev, generator=g).bfloat16(), torch.tensor([0.6], device=dev), torch.tensor([3.5], device=dev),
                      img_ids, torch.zeros(n_txt, 3, device=dev))
+    return eng, g, n_img, D
+
+
+def _alternate(eng, modes, kinds, rounds, per_round):
+    """Median / spread of the forward time (ms) of each (mode, kind), modes set by `modes[k]()`, alternating rounds."""
+    times = {(k, kind): [] for k in modes for kind in kinds}
+    for k, set_mode in modes.items():  # warm-up: every shape and every epilogue path
+        set_mode()
+        for kind in ("miss",) + tuple(kinds):
+            eng.forward(kind)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    for _ in range(rounds):
+        for k, set_mode in modes.items():
+            set_mode()
+            for kind in kinds:
+                torch.cuda.synchronize()
+                e0.record()
+                for _ in range(per_round):
+                    eng.forward(kind)
+                e1.record()
+                torch.cuda.synchronize()
+                times[(k, kind)].append(e0.elapsed_time(e1) / per_round)
+    return times
+
+
+def bench_controlnet(n_double, n_single, repeat, rounds, per_round):
+    """Miss forwards at the FLUX.1-dev 1024^2 shape (4096 image + 512 text tokens), without and with ControlNet samples,
+    alternating; the two outputs differ only through the samples."""
+    eng, g, n_img, D = _flux_1024_engine()
+    dev = eng.device
 
     def samples(n):
         return [(0.05 * torch.randn(1, n_img, D, device=dev, generator=g)).bfloat16() for _ in range(n)] if n else None
 
     ctrl = (samples(n_double), samples(n_single), repeat)
-    modes = {"plain": (None, None, False), "controlnet": ctrl}
-    times = {k: [] for k in modes}
-    for k, c in modes.items():  # warm-up: every shape and both epilogue paths
-        eng.stage_controlnet(*c)
-        eng.forward("miss")
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for _ in range(rounds):
-        for k, c in modes.items():
-            eng.stage_controlnet(*c)
-            torch.cuda.synchronize()
-            e0.record()
-            for _ in range(per_round):
-                eng.forward("miss")
-            e1.record()
-            torch.cuda.synchronize()
-            times[k].append(e0.elapsed_time(e1) / per_round)
+    modes = {"plain": lambda: eng.stage_controlnet(None, None, False), "controlnet": lambda: eng.stage_controlnet(*ctrl)}
+    times = {k: v for (k, _), v in _alternate(eng, modes, ("miss",), rounds, per_round).items()}
     n_reads = sum(x is not None for part in eng._controlnet_views() or () for x in part)
     name, power = card()
     med = {k: statistics.median(v) for k, v in times.items()}
@@ -77,6 +97,46 @@ def bench_controlnet(n_double, n_single, repeat, rounds, per_round):
                       "rounds": rounds, "forwards_per_round": per_round, "gpu": name, "power_limit": power}))
 
 
+def bench_lora(rank, rounds, per_round):
+    """Miss and hit forwards at the FLUX.1-dev 1024^2 shape without adapters and with one rank-`rank` adapter (scaling 1) on every
+    covered target, alternating."""
+    from magcache_b200.lora import LoraPack
+    eng, g, n_img, D = _flux_1024_engine()
+    w, dev = eng.w, eng.device
+
+    def ad(n_out, n_in):
+        A = (torch.randn(rank, n_in, device=dev, generator=g) / n_in ** 0.5).bfloat16()
+        return [(A, (0.02 * torch.randn(n_out, rank, device=dev, generator=g)).bfloat16(), 1.0)]
+
+    spec = {}
+    for i in range(len(w.double)):
+        for t, (o, k) in {"attn.to_q": (D, D), "attn.to_k": (D, D), "attn.to_v": (D, D), "attn.to_out.0": (D, D), "attn.add_q_proj": (D, D),
+                          "attn.add_k_proj": (D, D), "attn.add_v_proj": (D, D), "attn.to_add_out": (D, D), "ff.net.0.proj": (4 * D, D),
+                          "ff.net.2": (D, 4 * D), "ff_context.net.0.proj": (4 * D, D), "ff_context.net.2": (D, 4 * D),
+                          "norm1.linear": (6 * D, D), "norm1_context.linear": (6 * D, D)}.items():
+            spec[("double", i, t)] = ad(o, k)
+    for i in range(len(w.single)):
+        for t, (o, k) in {"attn.to_q": (D, D), "attn.to_k": (D, D), "attn.to_v": (D, D), "proj_mlp": (4 * D, D), "proj_out": (D, 5 * D),
+                          "norm.linear": (3 * D, D)}.items():
+            spec[("single", i, t)] = ad(o, k)
+    for t, (o, k) in {"x_embedder": (D, w.in_channels), "context_embedder": (D, w.joint_dim), "proj_out": (w.in_channels, D),
+                      "norm_out.linear": (2 * D, D)}.items():
+        spec[("top", 0, t)] = ad(o, k)
+    pack = LoraPack(w, spec)
+
+    def set_lora(p):
+        eng.lora = p
+
+    times = _alternate(eng, {"plain": lambda: set_lora(None), "lora": lambda: set_lora(pack)}, ("miss", "hit"), rounds, per_round)
+    name, power = card()
+    med = {f"ms_{k}_{kind}": round(statistics.median(v), 3) for (k, kind), v in times.items()}
+    print(json.dumps({"family": "flux", "workload": "1024x1024 forward", "lora_rank": rank, "lora_targets": len(spec), **med,
+                      "ms_added_miss": round(med["ms_lora_miss"] - med["ms_plain_miss"], 3),
+                      "ms_added_hit": round(med["ms_lora_hit"] - med["ms_plain_hit"], 3),
+                      "spread_ms": {f"{k}_{kind}": [round(min(v), 3), round(max(v), 3)] for (k, kind), v in times.items()},
+                      "rounds": rounds, "forwards_per_round": per_round, "gpu": name, "power_limit": power}))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("family", choices=["flux", "hunyuan"])
@@ -85,8 +145,14 @@ def main():
     ap.add_argument("--frames", type=int, default=33, help="hunyuan: latent frames (33 = 129 video frames)")
     ap.add_argument("--controlnet", default=None, help="flux: D,S double / single ControlNet samples; times the miss forward with and without")
     ap.add_argument("--controlnet-repeat", action="store_true", help="controlnet_blocks_repeat (XLabs): double block i reads sample i %% D")
-    ap.add_argument("--rounds", type=int, default=5, help="--controlnet: alternating rounds")
+    ap.add_argument("--lora", type=int, default=None, help="flux: rank of one adapter on every covered target; times miss and hit forwards with and without")
+    ap.add_argument("--rounds", type=int, default=5, help="--controlnet / --lora: alternating rounds")
     args = ap.parse_args()
+    if args.lora is not None:
+        if args.family != "flux":
+            ap.error("--lora is a FLUX option")
+        bench_lora(args.lora, args.rounds, args.steps or 10)
+        return
     if args.controlnet is not None:
         if args.family != "flux":
             ap.error("--controlnet is a FLUX option")
