@@ -169,6 +169,34 @@ def rope_table(ids, device, axes_dim=(16, 56, 56), theta=10000.0):
     return torch.tensor(cs.astype(np.float32)).to(device)  # torch-allocated (aligned) storage on every device
 
 
+class InputKey:
+    """Cache key of a table derived from a caller's tensors (RoPE positions, the valid length of a text mask). The tensors are held,
+    so their memory cannot go to another tensor while the key lives, and each is compared by storage, offset, shape, strides, dtype
+    and `_version`, which every torch write bumps (`copy_`, in-place ops, a write through any view). An address alone identifies
+    nothing: a caller that writes the next generation's ids into the same buffer keeps it, and so does the caching allocator when
+    it hands the freed block of one generation's mask to the next one's. Staging through a key adds no host synchronisation. Writes
+    torch does not see (through `.data`, DLPack or C, a CUDA graph replay into the tensor) keep the key: call `invalidate_engine`.
+
+    An inference tensor (made under `torch.inference_mode()`) has no version counter, and an in-place write to it inside inference
+    mode leaves no trace on the tensor. The key keeps a copy of such a tensor's content and compares it on every call: one small
+    comparison and one host synchronisation per call, for inference tensors only."""
+
+    __slots__ = ("held", "meta", "copies")
+
+    def __init__(self, *ts):
+        self.held, self.meta = ts, self._meta(ts)
+        self.copies = tuple(t.clone() if t.is_inference() else None for t in ts)
+
+    @staticmethod
+    def _meta(ts):
+        # a held storage stays allocated, so no other live storage can start at its address
+        return tuple((t.untyped_storage().data_ptr(), t.storage_offset(), tuple(t.shape), t.stride(), t.dtype, t.device,
+                      None if t.is_inference() else t._version) for t in ts)
+
+    def matches(self, *ts):
+        return self._meta(ts) == self.meta and all(c is None or torch.equal(c, t) for c, t in zip(self.copies, ts))
+
+
 def controlnet_index(i, n_blocks, n_samples, repeat=False):
     """Index of the ControlNet sample added after block `i` of `n_blocks`: the reference's expressions (magcache_flux.py:376-384 for
     the double blocks, `repeat` = XLabs' controlnet_blocks_repeat; :418-423 for the single blocks, which never repeat). The interval
@@ -489,11 +517,10 @@ class FluxEngine(MMDiTCore):
         tv = (timestep.reshape(-1)[:1].to(torch.bfloat16) * 1000).double()
         gv = (guidance.reshape(-1)[:1].to(torch.bfloat16) * 1000).double() if guidance is not None else torch.zeros(1, dtype=torch.float64, device=tv.device)
         self.s_t.copy_(torch.cat([tv, gv.to(tv.device)]))
-        key = (img_ids.data_ptr(), txt_ids.data_ptr(), n_img, n_txt)
-        if self._rope_key != key:  # ids are constant over a generation
+        if self._rope_key is None or not self._rope_key.matches(img_ids, txt_ids):  # ids are constant over a generation
             self._rope = rope_table(torch.cat((txt_ids.reshape(-1, 3), img_ids.reshape(-1, 3)), dim=0), self.device)  # :318
-            self._rope_key = key
-            assert self._rope.shape == (self.S_keys, 128)
+            self._rope_key = InputKey(img_ids, txt_ids)
+        assert self._rope.shape == (self.S_keys, 128)
 
     def stage_controlnet(self, block_samples, single_block_samples, blocks_repeat=False):
         """The call's ControlNet residuals (`controlnet_block_samples`, `controlnet_single_block_samples`,
@@ -735,13 +762,12 @@ class HunyuanEngine(MMDiTCore):
         assert x.shape[0] == 1 and text_states.shape[0] == 1, "one sample per call"
         _, c, ot, oh, ow = x.shape
         grid = (ot, oh // 2, ow // 2)
-        mkey = (text_mask.data_ptr(), tuple(text_mask.shape))
-        if self._mask_key != mkey:  # the mask is constant over a generation: one host read
+        if self._mask_key is None or not self._mask_key.matches(text_mask):  # the mask is constant over a generation: one host read
             m = text_mask.reshape(-1).to(torch.int64).cpu()
             valid = int(m.sum())
             if valid < 1 or not bool((m[:valid] == 1).all()):
                 raise NotImplementedError("magcache_b200: the valid text tokens must be a non-empty prefix of text_states (right padding)")
-            self._mask_key, self._valid = mkey, valid
+            self._mask_key, self._valid = InputKey(text_mask), valid
         n_txt = self._valid
         self._workspace(grid, n_txt)
         self.s_lat.copy_(x[0])
@@ -752,14 +778,13 @@ class HunyuanEngine(MMDiTCore):
         gv = guidance.reshape(-1)[:1].double() if guidance is not None else torch.zeros(1, dtype=torch.float64, device=t.device)
         self.s_t.copy_(torch.cat([t.reshape(-1)[:1].double(), gv.to(t.device)]))
         if freqs_cos is not None:
-            key = (freqs_cos.data_ptr(), freqs_sin.data_ptr(), self.n_img_total)
-            if self._rope_key != key:
-                n = self.n_img_total
-                assert tuple(freqs_cos.shape) == (n, 128) and tuple(freqs_sin.shape) == (n, 128)
+            n = self.n_img_total
+            assert tuple(freqs_cos.shape) == (n, 128) and tuple(freqs_sin.shape) == (n, 128)
+            if self._rope_key is None or not self._rope_key.matches(freqs_cos, freqs_sin):
                 cs = torch.stack([freqs_cos.float()[:, 0::2], freqs_sin.float()[:, 0::2]], dim=-1).reshape(n, 128)
-                self._rope, self._rope_key = cs.contiguous().to(self.device), key
+                self._rope, self._rope_key = cs.contiguous().to(self.device), InputKey(freqs_cos, freqs_sin)
         else:
-            self._rope = None
+            self._rope, self._rope_key = None, None
 
     # ------------------------------------------------------------------------------------------ token refiner (`self.txt_in`, :69)
     def _refine_text(self):

@@ -389,9 +389,11 @@ class OpenSoraEngine:
         self._tea_shape = self._shape
 
     def take_modulated_input(self, cur):
-        """Follow the `previous_modulated_input` attribute: None clears it; a tensor other than the engine's own buffer is copied in."""
+        """Follow the `previous_modulated_input` attribute: None clears it; a tensor other than the engine's own buffer is copied in.
+        One of another size is the previous generation's at another shape (the attribute outlives a generation, as in the reference,
+        which reads it on no forced call): there is no previous input."""
         self._tea_alloc()
-        if cur is None:
+        if cur is None or cur.numel() != self.mi[0].numel():
             self.mi_prev = None
         elif self.mi_prev is None or cur.data_ptr() != self.mi[self.mi_prev].data_ptr():
             self.mi_prev = 0 if self.mi_prev is None else self.mi_prev

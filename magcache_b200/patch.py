@@ -104,9 +104,10 @@ def _ctrl(self, family):
 def _take_residual(eng, cur, slot=None):
     """The reference keeps the cached residual in an attribute (`cur`, its current value); the engine keeps it in a fixed buffer that
     the attribute aliases (`eng.res`, or `eng.res[slot]` for the per-CFG-branch engines). If a caller replaced the attribute (or
-    cleared it), follow the attribute."""
+    cleared it), follow the attribute. A residual of another size is the previous generation's at another shape (the attribute
+    outlives a generation, as in the reference): it can serve no hit here, so the cache counts as empty."""
     res = eng.res if slot is None else eng.res[slot]
-    if cur is None:
+    if cur is None or (torch.is_tensor(cur) and cur.numel() != res.numel()):
         valid = False
     elif torch.is_tensor(cur) and cur.data_ptr() != res.data_ptr():
         res.copy_(cur.reshape(res.shape))
@@ -321,7 +322,10 @@ def reset_magcache(model):
     cls = model.__class__
     for attr in ("cnt", "accumulated_err", "accumulated_steps", "accumulated_ratio"):
         model.__dict__.pop(attr, None)
-    cls.cnt = 0
+    if torch.is_tensor(getattr(cls, "cnt", None)):
+        cls.cnt.fill_(0)  # Wan2.2's two experts share one counter tensor (MagCache4Wan2.2/magcache_generate.py:342): keep it shared
+    else:
+        cls.cnt = 0
     if isinstance(getattr(cls, "accumulated_err", None), list):
         cls.accumulated_err, cls.accumulated_steps, cls.accumulated_ratio = [0.0, 0.0], [0, 0], [1.0, 1.0]
     else:
@@ -675,8 +679,7 @@ def teacache_opensora_forward(self, x, timestep, all_timesteps, y, mask=None, x_
     calc = _TEA_OS.decide(self, forced, rel)  # :96-107
     self.previous_modulated_input = eng.mi[eng.mi_prev].view(eng.B, -1, eng.w.dim)  # :108 (every row, also under sequence parallelism)
     if not calc:
-        cur = self.previous_residual
-        _take_residual(eng, cur.reshape(eng.res.shape) if torch.is_tensor(cur) else cur)
+        _take_residual(eng, self.previous_residual)
     out = eng.forward_teacache(calc)
     if calc:
         self.previous_residual = eng.res.view(eng.B, eng.N, -1)  # :156
