@@ -260,6 +260,31 @@ int32_t mc_rmsnorm_rope_segs(void* x_bf16, int64_t ld, int64_t rows, int32_t seg
  * cos_sin: fp32 [rows, 128] interleaved (cos, sin) per pair, or NULL. */
 int32_t mc_rmsnorm_head_rope(void* x_bf16, int64_t ld, int64_t rows, int32_t heads, const float* w, float eps, const float* cos_sin,
                              void* stream);
+/* IP-Adapter image-prompt attention of one FLUX double block, every adapter in one launch (diffusers
+ * `FluxIPAdapterAttnProcessor` [EXT], reached through MagCache4FLUX/magcache_flux.py:321-324 and MagCache4FLUX_Kontext/
+ * magcache_flux_kontext.py:323-326; csrc/ip_attn.cu). For each image row i and head h:
+ *   qn     = bf16(bf16(q[i,h] * rsqrt(mean(q[i,h]^2) + eps)) * w)          the per-head RMSNorm of mc_rmsnorm_head_rope (same
+ *                                                                          code, same bits), without RoPE: `ip_query`
+ *   o_a    = softmax(qn K_a,h^T / sqrt(128)) V_a,h                          per adapter a, over its n_keys[a] keys, no mask
+ *   acc    = +0;  acc = bf16(acc + bf16(scales[a] * bf16(o_a)))  for a = 0 .. n_adapters-1 in order
+ *   out[i,h] = acc                                                          `ip_attn_output += scale * ...` from zeros_like
+ * o_a: fp32 scores from mma.sync, e = exp2f(log2(e) * (s - m) / sqrt(128)) with an online max over 64-key tiles, e ROUNDED TO
+ * BF16 for the PV product (fp32 accumulation), the row sum l over the unrounded e, o_a = bf16(acc_pv * (1 / l)). The sum starts
+ * at +0, so a -0 product (a zero scale, a zero output times a negative scale) leaves +0, as the reference's bf16 `+=` on
+ * zeros_like does. Readout bound: with V rows set to unit vectors the output of a key is P itself, and every such output is within
+ * 1.01 * 2^-7 * p + 2^-24 of p computed in fp64 from qn (two bf16 roundings of at most 2^-8 each: e and bf16(o_a); fp32 scores,
+ * exp2f and l add the 1 %).
+ * q: the raw q projection bf16 [rows, heads*128] (row pitch ldq: the q half of the fused q|k GEMM output, ldq = 2 * heads*128, or
+ * a q buffer of its own), read only; w fp32 [128] (the bf16 `norm_q.weight` values). kv bf16 (row pitch ldkv >= 2 * heads*128): the
+ * keys of adapter a are the n_keys[a] rows after those of adapters 0 .. a-1, K in columns [0, heads*128), V in [heads*128,
+ * 2*heads*128). n_keys / scales: host arrays of n_adapters entries. out bf16 [rows, heads*128] (row pitch ldo).
+ * Limits (MC_ERR_INVALID past them): 1 <= n_adapters <= MC_IP_ATTN_MAX_ADAPTERS, n_keys[a] >= 1, and the K and V rows of one head
+ * for all adapters staged in shared memory: sum_a ceil(n_keys[a] / 16) * 16 <= MC_IP_ATTN_MAX_KEYS. Pitches % 8 == 0, pointers
+ * 16-byte aligned. */
+#define MC_IP_ATTN_MAX_KEYS 384
+#define MC_IP_ATTN_MAX_ADAPTERS 8
+int32_t mc_ip_attn(const void* q, int64_t ldq, int64_t rows, int32_t heads, const float* w, float eps, const void* kv, int64_t ldkv,
+                   const int32_t* n_keys, const float* scales, int32_t n_adapters, void* out, int64_t ldo, void* stream);
 /* Open-Sora 1.2 (STDiT3, head_dim 72; csrc/opensora_kernels.cu) ------------------------------------------------------------
  * q / k normalisation of OpenSoraAttention.forward (videosys/models/modules/attentions.py:71-75, `qk_norm_legacy=False`): per-head
  * LlamaRMSNorm(72) (normalization.py:17-22: y = bf16(w * bf16(x * rsqrt(mean x^2 + eps))), w fp32 copies of the bf16 weight [72]),

@@ -9,13 +9,14 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmagcache_b200.so")
 SOURCES = ["controller.cu", "cache_kernels.cu", "rowwise_kernels.cu", "gemm_wgmma.cu", "attn_wgmma.cu", "head_wgmma.cu", "p2p.cu", "dit_forward.cu", "nccl_gather.cu", "opensora_kernels.cu",
-           "opensora_head.cu"]
+           "opensora_head.cu", "ip_attn.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
               "-Xptxas", "-v", "--expt-relaxed-constexpr"]
-# Entry functions that keep tensor-core accumulators in registers (wgmma; mma.sync for attn_varlen_d72_kernel and
-# attn_temporal_mma_d72_kernel) and must not spill. head_tc_kernel issues wgmma too but still spills (~350 B, in its
+# Entry functions that keep tensor-core accumulators in registers (wgmma; mma.sync for attn_varlen_d72_kernel,
+# attn_temporal_mma_d72_kernel and ip_attn_kernel) and must not spill. head_tc_kernel issues wgmma too but still spills (~350 B, in its
 # 104-register converter warps, not next to its accumulators); it joins this list once that is fixed (DESIGN §8).
-NO_SPILL_KERNELS = ("attn_kernel", "gemm_bf16_kernel", "attn_varlen_d72_kernel", "attn_temporal_mma_d72_kernel", "opensora_head_kernel")
+NO_SPILL_KERNELS = ("attn_kernel", "gemm_bf16_kernel", "attn_varlen_d72_kernel", "attn_temporal_mma_d72_kernel", "opensora_head_kernel",
+                    "ip_attn_kernel")
 
 
 def _nvcc():

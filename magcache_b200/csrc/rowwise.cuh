@@ -37,6 +37,24 @@ __device__ __forceinline__ float ln_rstd(const float (&v)[G][8], int lane, int l
   return rsqrtf(reduce(q) * inv_n + eps);
 }
 
+// Per-head RMSNorm (head_dim 128) of the q / k of the MMDiT attention, diffusers `RMSNorm(128)` with bf16 weight semantics:
+//   y = bf16(bf16(x * rsqrt(mean(x^2) + eps)) * w)
+// One head is held by a 16-lane segment (lanes 16s .. 16s + 15), 8 consecutive elements per lane in order; `w` points at this
+// lane's 8 weights. The sum of squares runs in lane order then over the segment by xor shuffles, so every caller gives the same
+// bits. Every lane of the warp must call it (full-mask shuffles).
+__device__ __forceinline__ void head_rmsnorm8(const float (&v)[8], const float* w, float eps, float (&o)[8]) {
+  float q = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) q = fmaf(v[j], v[j], q);
+#pragma unroll
+  for (int s = 8; s > 0; s >>= 1) q += __shfl_xor_sync(0xffffffffu, q, s);  // stays inside the 16-lane segment
+  const float r = rsqrtf(q * (1.0f / 128.0f) + eps);
+  float wv[8];
+  load_param8(w, wv);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) o[j] = round_bf16(round_bf16(v[j] * r) * wv[j]);
+}
+
 struct WarpReduce {  // the `reduce` of the warp-per-row forms
   __device__ __forceinline__ float operator()(float v) const { return warp_sum(v); }
 };

@@ -532,17 +532,9 @@ __global__ void __launch_bounds__(256) rmsnorm_head_rope_kernel(__nv_bfloat16* _
     __nv_bfloat16* px = x + row * ld + head * 128 + sub * 8;
     float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     if (live) unpack_bf16x8(*reinterpret_cast<const uint4*>(px), v);
-    float q = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) q = fmaf(v[j], v[j], q);
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);  // stays inside the 16-lane segment
+    float o[8];
+    head_rmsnorm8(v, w + sub * 8, eps, o);
     if (!live) continue;
-    const float r = rsqrtf(q * (1.0f / 128.0f) + eps);
-    float wv[8], o[8];
-    load_param8(w + sub * 8, wv);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) o[j] = round_bf16(round_bf16(v[j] * r) * wv[j]);
     if (cos_sin != nullptr) {
       float cs[8];
       ptx::ld_nc_v8_f32(cos_sin + row * 128 + sub * 8, cs);

@@ -29,6 +29,7 @@ import torch
 
 from . import _lib, ops
 from .lora import FluxLoraScan, LoraPack, Tailed, base_linear, is_lora_layer
+from .ops import IP_ATTN_MAX_ADAPTERS, IP_ATTN_MAX_KEYS
 
 E = _lib
 
@@ -205,16 +206,134 @@ def controlnet_index(i, n_blocks, n_samples, repeat=False):
     return i % n_samples if repeat else i // interval
 
 
+# diffusers' attention processors of a FLUX block, by class name (no diffusers import): the IP-Adapter processor (current name,
+# then the name before diffusers 0.32) and the plain ones, whose arithmetic the engine's blocks restate. The restated oracle
+# modules have no `processor` attribute.
+IP_PROCESSORS = ("FluxIPAdapterAttnProcessor", "FluxIPAdapterJointAttnProcessor2_0")
+PLAIN_PROCESSORS = ("FluxAttnProcessor", "FluxAttnProcessor2_0", "FluxAttnProcessor2_0_NPU")
+
+
+def ip_processor(attn, name):
+    """`attn.processor` when it is an IP-Adapter processor, None when the block runs the plain attention; any other processor
+    raises (its arithmetic is not the engine's)."""
+    proc = getattr(attn, "processor", None)
+    if proc is None or type(proc).__name__ in PLAIN_PROCESSORS:
+        return None
+    if type(proc).__name__ in IP_PROCESSORS:
+        return proc
+    raise NotImplementedError(f"magcache_b200: {name}.processor is a {type(proc).__name__}; the FLUX engine runs "
+                              f"{', '.join(PLAIN_PROCESSORS + IP_PROCESSORS)}")
+
+
+class IPAdapterCall:
+    """The IP-Adapter side path of one FLUX call, read from the module as it is at that call (processors, scales, weights):
+    `ip_hidden_states = encoder_hid_proj(ip_adapter_image_embeds)` (magcache_flux.py:321-324) and, in every double block with an
+    IP-Adapter processor, `ip_attn_output = sum_a scale[a] * SDPA(ip_query, to_k_ip[a](ip_h[a]), to_v_ip[a](ip_h[a]))` added to
+    the image stream after the feed-forward residual [EXT diffusers FluxIPAdapterAttnProcessor / FluxTransformerBlock]. Nothing
+    is kept between calls. The module's bf16 weights are read in place; only biases and norm parameters get fp32 copies."""
+
+    def __init__(self, module, procs, embeds, dim, device):
+        """`procs`: ip_processor() of each double block."""
+        name = "joint_attention_kwargs['ip_adapter_image_embeds']"
+        self.procs = procs
+        if not any(p is not None for p in self.procs):
+            raise NotImplementedError(f"magcache_b200: {name} given, but no double block has an IP-Adapter attention processor "
+                                      "(load the adapter with `load_ip_adapter`)")
+        if embeds is None:
+            raise NotImplementedError("magcache_b200: the model has IP-Adapter attention processors but the call passes no "
+                                      "ip_adapter_image_embeds (the reference's processor cannot run without them either)")
+        proj = getattr(module, "encoder_hid_proj", None)
+        self.layers = list(getattr(proj, "image_projection_layers", None) or ())
+        if not self.layers:
+            raise NotImplementedError("magcache_b200: IP-Adapter processors need `encoder_hid_proj` to be a "
+                                      "MultiIPAdapterImageProjection with its `image_projection_layers`")
+        lora_on = [f"encoder_hid_proj.{n}" for n, m in proj.named_modules() if is_lora_layer(m)]
+        for i, p in enumerate(self.procs):
+            if p is not None:
+                lora_on += [f"transformer_blocks.{i}.attn.processor.{k}.{a}" for k in ("to_k_ip", "to_v_ip")
+                            for a, m in enumerate(getattr(p, k)) if is_lora_layer(m)]
+        if lora_on:
+            raise NotImplementedError(f"magcache_b200: a LoRA adapter on the IP-Adapter's {lora_on[0]} is not supported")
+        A = len(self.layers)
+        if not isinstance(embeds, (list, tuple)) or len(embeds) != A:
+            raise NotImplementedError(f"magcache_b200: {name} must be a list of {A} tensors, one per loaded adapter; got "
+                                      f"{type(embeds).__name__}{'' if not isinstance(embeds, (list, tuple)) else f' of {len(embeds)}'}")
+        self.embeds, self.n_keys = [], []
+        for a, (e, layer) in enumerate(zip(embeds, self.layers)):
+            lin, norm = layer.image_embeds, layer.norm
+            want = (1, "num_images", lin.in_features)
+            if not (torch.is_tensor(e) and e.dim() == 3 and e.shape[0] == 1 and e.shape[1] >= 1 and e.shape[2] == lin.in_features
+                    and e.dtype == torch.bfloat16 and e.device == device):
+                got = f"{e.dtype} {tuple(e.shape)} on {e.device}" if torch.is_tensor(e) else type(e).__name__
+                raise NotImplementedError(f"magcache_b200: {name}[{a}] must be a bf16 tensor of shape {list(want)} on {device} "
+                                          f"(one sample per call); got {got}")
+            C = norm.normalized_shape[0]
+            if norm.weight is None or norm.bias is None or lin.out_features != layer.num_image_text_embeds * C:
+                raise NotImplementedError(f"magcache_b200: encoder_hid_proj.image_projection_layers[{a}] is not an ImageProjection "
+                                          "(Linear to num_image_text_embeds x C, affine LayerNorm(C))")
+            self.embeds.append(e[0].contiguous())
+            self.n_keys.append(e.shape[1] * layer.num_image_text_embeds)
+        if A > IP_ATTN_MAX_ADAPTERS or sum((n + 15) // 16 * 16 for n in self.n_keys) > IP_ATTN_MAX_KEYS:
+            raise NotImplementedError(f"magcache_b200: {A} IP-Adapters with {self.n_keys} image-prompt tokens: the kernel holds at most "
+                                      f"{IP_ATTN_MAX_ADAPTERS} adapters and {IP_ATTN_MAX_KEYS} tokens (each adapter's count "
+                                      "rounded up to 16)")
+        self.scales = []
+        for i, p in enumerate(self.procs):
+            if p is None:
+                self.scales.append(None)
+                continue
+            s = list(p.scale) if isinstance(p.scale, (list, tuple)) else [p.scale]
+            if not (len(s) == len(p.to_k_ip) == len(p.to_v_ip) == A):
+                raise NotImplementedError(f"magcache_b200: transformer_blocks.{i}.attn.processor has {len(s)} scales, {len(p.to_k_ip)} "
+                                          f"to_k_ip and {len(p.to_v_ip)} to_v_ip for {A} image projections")
+            for lin in list(p.to_k_ip) + list(p.to_v_ip):
+                wt = lin.weight
+                if not (wt.dtype == torch.bfloat16 and wt.device == device and wt.shape == (dim, self.layers[0].norm.normalized_shape[0])
+                        and wt.stride(1) == 1 and wt.stride(0) % 8 == 0):
+                    raise NotImplementedError(f"magcache_b200: transformer_blocks.{i}.attn.processor weights must be bf16 "
+                                              f"[{dim}, C] on {device}; got {wt.dtype} {tuple(wt.shape)} on {wt.device}")
+            self.scales.append([float(x) for x in s])
+        self.dim, self.device = dim, device
+
+    def project(self):
+        """`encoder_hid_proj(ip_adapter_image_embeds)`: per adapter LayerNorm(Linear(x).reshape(num_images * T, C)), on the GEMM
+        and LayerNorm kernels. Returns the per-block launches for `MMDiTCore.run_blocks`."""
+        f32 = torch.float32
+        self.hidden = []
+        for x, layer in zip(self.embeds, self.layers):
+            lin, norm = layer.image_embeds, layer.norm
+            y = ops.gemm(x, lin.weight, None if lin.bias is None else ops.cast(lin.bias, f32), E.MC_EPI_BIAS_BF16)
+            y = y.view(-1, norm.normalized_shape[0])
+            self.hidden.append(ops.ln_affine(y, ops.cast(norm.weight, f32), ops.cast(norm.bias, f32), eps=norm.eps))
+        self.kv = torch.empty(sum(self.n_keys), 2 * self.dim, dtype=torch.bfloat16, device=self.device)
+        return [None if p is None else (lambda q, nq, heads, out, i=i: self.attend(i, q, nq, heads, out)) for i, p in enumerate(self.procs)]
+
+    def attend(self, i, q, nq, heads, out):
+        """Double block `i`: every adapter's K | V rows from its `to_k_ip` / `to_v_ip`, then `mc_ip_attn` on the raw q into `out`."""
+        D, f32, k0 = self.dim, torch.float32, 0
+        p = self.procs[i]
+        for h, n, tk, tv in zip(self.hidden, self.n_keys, p.to_k_ip, p.to_v_ip):
+            for lin, cols in ((tk, slice(0, D)), (tv, slice(D, 2 * D))):
+                ops.gemm(h, lin.weight, None if lin.bias is None else ops.cast(lin.bias, f32), E.MC_EPI_BIAS_BF16, out=self.kv[k0:k0 + n, cols])
+            k0 += n
+        ops.ip_attention(q, nq, heads, self.kv, self.n_keys, self.scales[i], out=out)
+
+
 class MMDiTCore:
     """Workspace + block stack shared by the FLUX and HunyuanVideo engines. A subclass provides `self.w` (dim, heads, double, single,
     ada_w / ada_b / ada_rows), the token order (`txt_first`), the RoPE table of the rows that get RoPE, and its own prologue / head."""
 
     txt_first = True
     lora = None  # lora.LoraPack of the current call (FLUX with unmerged adapters), else None
+    ip = None    # IPAdapterCall of the current call (FLUX with IP-Adapter processors), else None
 
     def _controlnet_views(self):
         """`run_blocks`' ControlNet argument for the current call; only the FLUX engine takes ControlNet residuals."""
         return None
+
+    def _ip_blocks(self):
+        """`run_blocks`' IP-Adapter argument for the current call (the image projection runs here, on a miss or calibration call only)."""
+        return None if self.ip is None else self.ip.project()
 
     def _alloc_core(self, n_img, n_txt):
         """Buffers for one (image tokens, text tokens) shape. Token-sharded (`self.world > 1`, SURVEY §8e): the IMAGE rows are split over
@@ -351,21 +470,27 @@ class MMDiTCore:
         gather_rows(o_local.contiguous(), full, self.shard.group)
         return full
 
-    def run_blocks(self, ctrl=None):
+    def run_blocks(self, ctrl=None, ip=None):
         """Double-stream then single-stream blocks (magcache_flux.py:343-424; magcache_sample_video.py:108-139) on `hs`; the image rows of
         `hs` must hold the embedded image tokens and the text rows the embedded text. Returns the image rows.
 
         `ctrl`: None, or (double, single) lists with one entry per block — a bf16 [n_img, D] view (this rank's image rows) added to
         the image stream after that block (FLUX ControlNet residuals, magcache_flux.py:374-384 / :416-423), or None. The addition is
         fused into the block's last GEMM on the image rows (MC_EPI_BIAS_GATE_RESID_ADD_BF16): FF2 of the image stream of a double
-        block, the `out` GEMM of a single block from row n_txt on (text rows first, FLUX only)."""
+        block, the `out` GEMM of a single block from row n_txt on (text rows first, FLUX only).
+
+        `ip`: None, or one entry per double block — None, or `f(q, norm_q weight, heads, out)` writing the block's IP-Adapter
+        attention output (IPAdapterCall.attend) from the raw q of this rank's image rows, before `_qk_norm` overwrites q. The
+        output goes to cat[img, :D] (free in double blocks) and is added after the image stream's feed-forward residual as FF2's
+        addend; a ControlNet sample of the same block is added afterwards in its own bf16 add, the reference's order."""
         w, D, S = self.w, self.w.dim, self.S
         double, single = (w.double, w.single) if self.lora is None else (self.lora.double, self.lora.single)
         c_double, c_single = ctrl if ctrl is not None else ((None,) * len(w.double), (None,) * len(w.single))
+        c_ip = ip if ip is not None else (None,) * len(w.double)
         txt, img = self.txt, self.img
         hs, h = self.hs, self.h
         down = self._down
-        for b, add in zip(double, c_double):
+        for b, add, ipf in zip(double, c_double, c_ip):
             lg = b.get("lora", {})  # this block's LoRA down-projections, keyed by the GEMM input they read
             em, emc = self._em(b["ada"], 6), self._em(b["ada_c"], 6)  # (shift1, scale1, gate1, shift2, scale2, gate2)
             ops.ln_modulate(hs[img], em, 1, 0, round_ln_to_bf16=True, out=h[img])
@@ -374,6 +499,10 @@ class MMDiTCore:
             down(lg, "ch", h[txt])
             self._project(img, h[img], b["qk_w"], b["qk_b"], b["v_w"], b["v_b"])
             self._project(txt, h[txt], b["cqk_w"], b["cqk_b"], b["cv_w"], b["cv_b"])
+            ip_out = None
+            if ipf is not None:
+                ip_out = self.cat[img][:, :D]
+                ipf(self.qk[img][:, :D] if self.shard is None else self.q_loc[img], b["nq"], w.heads, ip_out)
             self._qk_norm(img, b["nq"], b["nk"])
             self._qk_norm(txt, b["cnq"], b["cnk"])
             self._joint_attention(self.att)
@@ -388,7 +517,12 @@ class MMDiTCore:
                 ffh = self.cat[rows][:, D:]
                 self._linear(h[rows], f1w, f1b, E.MC_EPI_BIAS_GELU_BF16, out=ffh)
                 down(lg, pre + "ffh", ffh)
-                self._linear(ffh, f2w, f2b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[rows], gate=e[5], addend=add if rows == img else None)
+                if rows != img:
+                    self._linear(ffh, f2w, f2b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[rows], gate=e[5])
+                    continue
+                self._linear(ffh, f2w, f2b, E.MC_EPI_BIAS_GATE_RESID_BF16, out=hs[rows], gate=e[5], addend=add if ip_out is None else ip_out)
+                if ip_out is not None and add is not None:
+                    ops.cache_hit_add(hs[img], add.contiguous(), out=hs[img])
         allr = slice(0, S)
         for b, add in zip(single, c_single):
             lg = b.get("lora", {})
@@ -423,7 +557,7 @@ class MMDiTCore:
             x = ops.cache_hit_add(x0, self.res, out=self.hit)                     # magcache_flux.py:340 ; magcache_sample_video.py:104
         else:
             self.hs[self.img].copy_(x0)                                           # `ori_hidden_states` / `ori_img` stays in x0
-            x = self.run_blocks(self._controlnet_views())
+            x = self.run_blocks(self._controlnet_views(), self._ip_blocks())
             if self.shard is not None:
                 self.xch.join()  # every push of this forward is ordered before its end
             ops.residual_sub(x.contiguous(), x0, out=self.res)                    # :426 ; :140 (x is a contiguous row range of hs)
@@ -438,7 +572,7 @@ class MMDiTCore:
         multiples of 2^-8 (the shipped FLUX table is visibly bf16-quantised, SURVEY §8a row 9)."""
         x0 = self.prologue()
         self.hs[self.img].copy_(x0)
-        x = self.run_blocks(self._controlnet_views())
+        x = self.run_blocks(self._controlnet_views(), self._ip_blocks())
         reduce = None
         if self.shard is not None:  # the statistics are sums over the image tokens: add the partial sums of every token shard
             from .shard import allreduce_stats
@@ -463,6 +597,7 @@ class FluxEngine(MMDiTCore):
         self.res_valid = False
         self.controlnet = (None, None, False)
         self._lora_scan, self._lora_merged, self._lora_wrappers = None, (), ()
+        self.ip = None
 
     def sync_lora(self, module):
         """Take the module's unmerged LoRA adapters as they are now (lora.FluxLoraScan): called at every forward, after the
@@ -527,6 +662,19 @@ class FluxEngine(MMDiTCore):
         `controlnet_blocks_repeat`). Kept as given: they are validated and read only when the block stack runs (a miss or a
         calibration call); a hit ignores them, as the reference does."""
         self.controlnet = (block_samples, single_block_samples, bool(blocks_repeat))
+
+    def stage_ip_adapter(self, module, embeds):
+        """The call's IP-Adapter side path: the module's processors, scales and weights as they are now, and the call's
+        `ip_adapter_image_embeds` (or None). Checked here, on every call; the projections run only when the block stack runs (a
+        hit cannot reach their output). A model without IP-Adapter processors and a call without embeds stage nothing."""
+        procs = [ip_processor(b.attn, f"transformer_blocks.{i}.attn") for i, b in enumerate(module.transformer_blocks)]
+        for i, b in enumerate(module.single_transformer_blocks):
+            if ip_processor(b.attn, f"single_transformer_blocks.{i}.attn") is not None:
+                raise NotImplementedError(f"magcache_b200: single_transformer_blocks.{i}.attn has an IP-Adapter processor; FLUX's "
+                                          "single blocks take no image prompt")
+        self.ip = None
+        if embeds is not None or any(p is not None for p in procs):
+            self.ip = IPAdapterCall(module, procs, embeds, self.w.dim, self.device)
 
     def _controlnet_sample(self, sample, what):
         """This rank's rows of one sample as a [n_img, D] view (no copy). Only a CUDA bf16 [1, n_img, D] tensor with unit column

@@ -263,6 +263,37 @@ def rmsnorm_head_rope_(x, weight, heads, cos_sin=None, eps=1e-6, tag=None):
     return x
 
 
+IP_ATTN_MAX_KEYS, IP_ATTN_MAX_ADAPTERS = 384, 8  # MC_IP_ATTN_MAX_KEYS / MC_IP_ATTN_MAX_ADAPTERS
+
+
+def ip_attention(q, weight, heads, kv, n_keys, scales, out=None, eps=1e-6, tag=None):
+    """IP-Adapter image-prompt attention of one FLUX double block over every adapter (`mc_ip_attn`): the per-head RMSNorm of the
+    raw q projection (`weight` fp32 [128], no RoPE), then per adapter a, in order, acc = bf16(acc + bf16(scales[a] *
+    bf16(softmax(qn K_a^T / sqrt(128)) V_a))) from +0. q bf16 [rows, heads*128] (row stride allowed, read only); kv bf16
+    [sum(n_keys), >= 2*heads*128]: adapter a's K | V rows follow those of the adapters before it. Raises NotImplementedError past
+    the kernel's limits: IP_ATTN_MAX_ADAPTERS adapters, IP_ATTN_MAX_KEYS key rows per head with each count rounded up to 16."""
+    import ctypes
+    _dev(q), _dev(kv)
+    D = heads * 128
+    n_keys, scales = [int(n) for n in n_keys], [float(s) for s in scales]
+    assert q.dtype == kv.dtype == torch.bfloat16 and q.dim() == 2 and q.shape[1] == D and q.stride(1) == 1 and kv.stride(1) == 1
+    assert weight.dtype == torch.float32 and weight.numel() == 128 and weight.is_contiguous()
+    assert len(n_keys) == len(scales) >= 1 and min(n_keys) >= 1 and kv.shape == (sum(n_keys), kv.shape[1]) and kv.shape[1] >= 2 * D
+    if len(n_keys) > IP_ATTN_MAX_ADAPTERS or sum((n + 15) // 16 * 16 for n in n_keys) > IP_ATTN_MAX_KEYS:
+        raise NotImplementedError(f"magcache_b200: IP-Adapter attention over {len(n_keys)} adapters with {n_keys} keys: the kernel "
+                                  f"holds at most {IP_ATTN_MAX_ADAPTERS} adapters and {IP_ATTN_MAX_KEYS} key rows per head (each "
+                                  "adapter's count rounded up to 16)")
+    if out is None:
+        out = torch.empty(q.shape[0], D, dtype=torch.bfloat16, device=q.device)
+    assert out.dtype == torch.bfloat16 and out.shape == q.shape and out.stride(1) == 1
+    nk, sc = (ctypes.c_int32 * len(n_keys))(*n_keys), (ctypes.c_float * len(scales))(*scales)
+    with _Timed(tag, "ip_attn"):
+        check(lib.mc_ip_attn(q.data_ptr(), q.stride(0), q.shape[0], heads, weight.data_ptr(), eps, kv.data_ptr(), kv.stride(0), nk, sc,
+                             len(n_keys), out.data_ptr(), out.stride(0), _stream()))
+    _count()
+    return out
+
+
 def rmsnorm_head72_rope_(x, weight, heads, cos_sin=None, pos_div=1, eps=1e-6, tag=None):
     """In-place per-head LlamaRMSNorm(72) + optional RoPE (`mc_rmsnorm_head72_rope`) on a bf16 [rows, heads*72] view (row stride
     allowed): the q / k normalisation of Open-Sora's attention. weight fp32 [72]; cos_sin fp32 [P, 72] (interleaved cos, sin per pair),

@@ -384,11 +384,12 @@ class _Sample:
 
 
 def _flux_lora_scale(self, hidden_states, joint_attention_kwargs):
-    """The call's LoRA scale (:274-279), after the checks that need no engine: only a "scale" key is built, CUDA inputs only."""
-    extra = sorted(k for k in (joint_attention_kwargs or {}) if k != "scale")
+    """The call's LoRA scale (:274-279), after the checks that need no engine: only the "scale" and "ip_adapter_image_embeds"
+    keys are built, CUDA inputs only."""
+    extra = sorted(k for k in (joint_attention_kwargs or {}) if k not in ("scale", "ip_adapter_image_embeds"))
     if extra:
-        raise NotImplementedError(f"magcache_b200: joint_attention_kwargs {extra} (ip-adapter, ...) are not built for the FLUX engine; "
-                                  "only the LoRA 'scale' is")
+        raise NotImplementedError(f"magcache_b200: joint_attention_kwargs {extra} are not built for the FLUX engine; only the LoRA "
+                                  "'scale' and 'ip_adapter_image_embeds' are")
     if not hidden_states.is_cuda:
         raise RuntimeError("magcache_b200: hidden_states must be CUDA tensors (no CPU path)")
     lora_scale = joint_attention_kwargs.get("scale", 1.0) if joint_attention_kwargs is not None else 1.0
@@ -411,12 +412,13 @@ def _lora_scaled(self, lora_scale):
 
 
 def _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
-                controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat):
+                controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat, joint_attention_kwargs):
     """Stages one FLUX call on the engine (inside `_lora_scaled`) and hands it the adapters as they are now."""
     is_module = isinstance(self, torch.nn.Module)
     eng = _cached_engine(self, "_mc_flux_engine", lambda **kw: FluxEngine(FluxWeights.from_module(self, hidden_states.device), **kw))
-    if is_module:  # (a benchmark's MMDiTHandle sets the engine's LoRA pack itself)
+    if is_module:  # (a benchmark's MMDiTHandle sets the engine's LoRA pack and IP-Adapter call itself)
         eng.sync_lora(self)
+        eng.stage_ip_adapter(self, (joint_attention_kwargs or {}).get("ip_adapter_image_embeds"))
     if txt_ids.ndim == 3:  # :305-316 (deprecated 3-D ids)
         txt_ids = txt_ids[0]
     if img_ids.ndim == 3:
@@ -434,11 +436,13 @@ def magcache_flux_forward(self, hidden_states, encoder_hidden_states=None, poole
     with `.sample`. ControlNet residuals (:374-384, :416-423) are added after their blocks on a miss, fused into each block's last GEMM
     on the image rows; a hit ignores them, as the reference does. Unmerged PEFT LoRA adapters run as tails of the GEMMs of the
     Linears they adapt (magcache_b200/lora.py), scaled by `joint_attention_kwargs["scale"]` with the reference's
-    scale / unscale statements (:274-287, :437-439) on every call, hit or miss. ip-adapter (:321-324) is not built and raises."""
+    scale / unscale statements (:274-287, :437-439) on every call, hit or miss. IP-Adapter image prompts
+    (`joint_attention_kwargs["ip_adapter_image_embeds"]`, :321-324) run on a miss: the image projection, then per double block
+    one `mc_ip_attn` launch whose output FF2's epilogue adds (mmdit.IPAdapterCall); a hit ignores them."""
     lora_scale = _flux_lora_scale(self, hidden_states, joint_attention_kwargs)
     with _lora_scaled(self, lora_scale):
         eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
-                          controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat)
+                          controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat, joint_attention_kwargs)
         ctrl = _ctrl(self, "flux")
         skip_forward = ctrl.decide(self)  # :326-338
         _take_residual(eng, self.previous_residual)
@@ -457,11 +461,12 @@ def magcache_flux_calibration(self, hidden_states, encoder_hidden_states=None, p
     r"""MagCache4FLUX/magcache_flux.py:21-231: every call runs the block stack and, from the second call on, records the token-mean
     magnitude ratio, its std and the cosine distance to the previous residual (`norm_ratio / norm_std / cos_dis`, rounded to 5 places);
     the lists are printed on the last call of a generation and cleared at the wrap (:207-221). ControlNet residuals as in the
-    forward (:145-155, :187-193); LoRA adapters and scale as in the forward (:62-75, :224-226); ip-adapter raises."""
+    forward (:145-155, :187-193); LoRA adapters and scale as in the forward (:62-75, :224-226); IP-Adapter image prompts as in the
+    forward (:108-111)."""
     lora_scale = _flux_lora_scale(self, hidden_states, joint_attention_kwargs)
     with _lora_scaled(self, lora_scale):
         eng = _flux_stage(self, hidden_states, encoder_hidden_states, pooled_projections, timestep, img_ids, txt_ids, guidance,
-                          controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat)
+                          controlnet_block_samples, controlnet_single_block_samples, controlnet_blocks_repeat, joint_attention_kwargs)
         if self.cnt == 0:
             eng.res_valid = False  # `if self.cnt>=1` (:199): the first call of a generation has nothing to compare with
         out, stats = eng.calibrate()

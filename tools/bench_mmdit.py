@@ -5,6 +5,7 @@ Not the contract bench (bench.py measures the north-star Wan2.1 workload); writt
 usage (GPU): python tools/bench_mmdit.py flux|hunyuan [--steps N] [--no-cache] [--tokens-scale F]
              python tools/bench_mmdit.py flux --controlnet D,S [--controlnet-repeat] [--rounds R] [--steps N]
              python tools/bench_mmdit.py flux --lora RANK [--rounds R] [--steps N]
+             python tools/bench_mmdit.py flux --ip-adapter A[,T] [--rounds R] [--steps N]
 
 --controlnet D,S: the FLUX 1024^2 miss forward (the whole block stack) with D double-block and S single-block synthetic bf16
 ControlNet samples (S = 0: none for the single blocks) against the same forward without samples, timed in alternating rounds of N
@@ -12,7 +13,11 @@ forwards each with CUDA events; prints the card name and power limit beside the 
 
 --lora RANK: the FLUX 1024^2 miss and hit forwards with one synthetic rank-RANK LoRA adapter on every covered target (every block
 Linear, every AdaLayerNorm projection, x_embedder, context_embedder, proj_out; magcache_b200/lora.py) against the same forwards
-without adapters, alternating rounds as for --controlnet."""
+without adapters, alternating rounds as for --controlnet.
+
+--ip-adapter A[,T]: the FLUX 1024^2 miss and hit forwards with A synthetic XLabs-shaped IP-Adapters (768-wide image embeds projected
+to T tokens of 4096, default T = 16; `to_k_ip` / `to_v_ip` on all 19 double blocks) against the same forwards without them,
+alternating rounds as for --controlnet; then `mc_ip_attn` alone at 4096 rows with its bytes per launch and rate."""
 import argparse
 import json
 import os
@@ -137,6 +142,73 @@ def bench_lora(rank, rounds, per_round):
                       "rounds": rounds, "forwards_per_round": per_round, "gpu": name, "power_limit": power}))
 
 
+class FluxIPAdapterAttnProcessor(torch.nn.Module):
+    """diffusers' processor surface the engine reads (its class name, `to_k_ip`, `to_v_ip`, `scale`)."""
+
+    def __init__(self, D, C, n, dev):
+        super().__init__()
+        kw = dict(device=dev, dtype=torch.bfloat16)
+        self.to_k_ip = torch.nn.ModuleList([torch.nn.Linear(C, D, **kw) for _ in range(n)])
+        self.to_v_ip = torch.nn.ModuleList([torch.nn.Linear(C, D, **kw) for _ in range(n)])
+        self.scale = [1.0] * n
+
+
+def bench_ip_adapter(n_adapters, T, rounds, per_round):
+    """Miss and hit forwards at the FLUX.1-dev 1024^2 shape without and with `n_adapters` IP-Adapters of T tokens, alternating;
+    then the kernel alone."""
+    import types
+    eng, g, n_img, D = _flux_1024_engine()
+    dev, C, emb = eng.device, 4096, 768
+    kw = dict(device=dev, dtype=torch.bfloat16)
+    with torch.no_grad():
+        layers = torch.nn.ModuleList()
+        for _ in range(n_adapters):
+            layer = torch.nn.Module()
+            layer.image_embeds, layer.norm, layer.num_image_text_embeds = torch.nn.Linear(emb, T * C, **kw), torch.nn.LayerNorm(C, **kw), T
+            layers.append(layer)
+        proj = torch.nn.Module()
+        proj.image_projection_layers = layers
+        procs = [FluxIPAdapterAttnProcessor(D, C, n_adapters, dev) for _ in eng.w.double]
+        for p in list(proj.parameters()) + [q for pr in procs for q in pr.parameters()]:
+            if p.dim() == 2:
+                p.normal_(0.0, p.shape[1] ** -0.5, generator=g)
+    module = types.SimpleNamespace(encoder_hid_proj=proj)
+    embeds = [torch.randn(1, 1, emb, device=dev, generator=g).bfloat16() for _ in range(n_adapters)]
+    call = mmdit.IPAdapterCall(module, procs, embeds, D, dev)
+
+    def set_ip(c):
+        eng.ip = c
+
+    times = _alternate(eng, {"plain": lambda: set_ip(None), "ip": lambda: set_ip(call)}, ("miss", "hit"), rounds, per_round)
+    # the kernel alone at 4096 rows: q the q half of a q|k buffer, out the 5D-pitch buffer the engine writes
+    q = torch.randn(n_img, 2 * D, device=dev, generator=g).bfloat16()[:, :D]
+    out = torch.empty(n_img, 5 * D, **kw)[:, :D]
+    kv = torch.randn(n_adapters * T, 2 * D, device=dev, generator=g).bfloat16()
+    w = torch.ones(128, device=dev)
+    args = (q, w, eng.w.heads, kv, [T] * n_adapters, [1.0] * n_adapters)
+    for _ in range(10):
+        ops.ip_attention(*args, out=out)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    n = 200
+    torch.cuda.synchronize()
+    e0.record()
+    for _ in range(n):
+        ops.ip_attention(*args, out=out)
+    e1.record()
+    torch.cuda.synchronize()
+    us = e0.elapsed_time(e1) / n * 1e3
+    kernel_bytes = 2 * n_img * D * 2 + n_adapters * T * 2 * D * 2  # q read, output written, K|V read once per head (L2 after that)
+    name, power = card()
+    med = {f"ms_{k}_{kind}": round(statistics.median(v), 3) for (k, kind), v in times.items()}
+    print(json.dumps({"family": "flux", "workload": "1024x1024 forward", "ip_adapters": n_adapters, "ip_tokens": T, **med,
+                      "ms_added_miss": round(med["ms_ip_miss"] - med["ms_plain_miss"], 3),
+                      "ms_added_hit": round(med["ms_ip_hit"] - med["ms_plain_hit"], 3),
+                      "spread_ms": {f"{k}_{kind}": [round(min(v), 3), round(max(v), 3)] for (k, kind), v in times.items()},
+                      "ip_attn_us_4096_rows": round(us, 2), "ip_attn_bytes": kernel_bytes,
+                      "ip_attn_GBps": round(kernel_bytes / (us * 1e-6) / 1e9, 1),
+                      "rounds": rounds, "forwards_per_round": per_round, "gpu": name, "power_limit": power}))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("family", choices=["flux", "hunyuan"])
@@ -146,8 +218,15 @@ def main():
     ap.add_argument("--controlnet", default=None, help="flux: D,S double / single ControlNet samples; times the miss forward with and without")
     ap.add_argument("--controlnet-repeat", action="store_true", help="controlnet_blocks_repeat (XLabs): double block i reads sample i %% D")
     ap.add_argument("--lora", type=int, default=None, help="flux: rank of one adapter on every covered target; times miss and hit forwards with and without")
-    ap.add_argument("--rounds", type=int, default=5, help="--controlnet / --lora: alternating rounds")
+    ap.add_argument("--ip-adapter", default=None, help="flux: A[,T] IP-Adapters of T image-prompt tokens (default 16); times miss and hit forwards with and without")
+    ap.add_argument("--rounds", type=int, default=5, help="--controlnet / --lora / --ip-adapter: alternating rounds")
     args = ap.parse_args()
+    if args.ip_adapter is not None:
+        if args.family != "flux":
+            ap.error("--ip-adapter is a FLUX option")
+        a_t = [int(v) for v in args.ip_adapter.split(",")]
+        bench_ip_adapter(a_t[0], a_t[1] if len(a_t) > 1 else 16, args.rounds, args.steps or 10)
+        return
     if args.lora is not None:
         if args.family != "flux":
             ap.error("--lora is a FLUX option")
