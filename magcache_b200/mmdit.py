@@ -429,7 +429,11 @@ class MMDiTCore:
                 self._linear(hp, qk_w[D:], qk_b[D:], E.MC_EPI_BIAS_BF16, out=dst[:, :D])
                 self._linear(hp, v_w, v_b, E.MC_EPI_BIAS_BF16, out=dst[:, D:])
             return
-        self._linear(h_rows, qk_w, qk_b, E.MC_EPI_BIAS_BF16, out=self.qk[rows])
+        if isinstance(qk_w, tuple):  # (q, k) weights read in place (QwenImageWeights): one GEMM into each half of qk
+            for i, wt in enumerate(qk_w):
+                self._linear(h_rows, wt, qk_b[i * D:(i + 1) * D], E.MC_EPI_BIAS_BF16, out=self.qk[rows][:, i * D:(i + 1) * D])
+        else:
+            self._linear(h_rows, qk_w, qk_b, E.MC_EPI_BIAS_BF16, out=self.qk[rows])
         self._linear(h_rows, v_w, v_b, E.MC_EPI_BIAS_BF16, out=self.v[rows])
 
     def _qk_norm(self, rows, nq, nk):
@@ -991,6 +995,259 @@ class HunyuanEngine(MMDiTCore):
 
 
 # ======================================================================================================================
+# Qwen-Image / Qwen-Image-Edit
+# ======================================================================================================================
+class QwenImageWeights:
+    """Weights of one QwenImageTransformer2DModel (diffusers attribute names). Its 60 double blocks are FLUX double blocks statement
+    for statement (per-stream `Linear(silu(temb))` -> (shift, scale, gate) x 2, LayerNorm without affine at eps 1e-6, biased
+    q/k/v/o, per-head RMSNorm of q and k, interleaved-pair RoPE, joint attention over [txt | img], GELU(tanh) FF at 4 D), so they
+    run on `MMDiTCore.run_blocks` with no single blocks.
+
+    At 20 B parameters (40.9 GB in bf16) nothing large is copied: every block matrix is the module's own bf16 weight, read in
+    place. The modulation rows stay one part per Linear (`ada_parts`; a stacked copy would be 13.6 GB), and q and k run as two
+    GEMMs into the halves of `qk` instead of one over a fused q|k copy (4.5 GB): 240 more GEMM launches per miss, each over half
+    the columns. The engine's own copies are the biases and norm weights, as fp32 (22 MB at full size)."""
+
+    fp8_scratch = None
+
+    def __init__(self):
+        self.double, self.single = [], []
+
+    @classmethod
+    def from_module(cls, m, dev):
+        for name, mod in m.named_modules():
+            if is_lora_layer(mod):
+                raise NotImplementedError(f"magcache_b200: the Qwen-Image engine runs no LoRA adapters; {name} carries one "
+                                          "(merge it into the weights first)")
+        cfg = m.config
+        if cfg.attention_head_dim != 128 or tuple(cfg.axes_dims_rope) != (16, 56, 56):
+            raise NotImplementedError("magcache_b200: the Qwen-Image engine needs head_dim 128 with RoPE axes (16, 56, 56)")
+        if getattr(cfg, "guidance_embeds", False):
+            raise NotImplementedError("magcache_b200: Qwen-Image with guidance_embeds is not supported (the released checkpoints have none)")
+        for name, p in m.named_parameters():
+            if p.dtype != torch.bfloat16 or p.device != dev:
+                raise NotImplementedError(f"magcache_b200: the Qwen-Image engine reads the module's bf16 weights in place on {dev}; "
+                                          f"{name} is {p.dtype} on {p.device}")
+        w = cls()
+        w.heads = cfg.num_attention_heads
+        w.dim = D = w.heads * 128
+        w.in_channels, w.joint_dim = cfg.in_channels, cfg.joint_attention_dim
+        v = lambda t: t.detach()  # noqa: E731  (the module's own storage)
+
+        def lin(l):
+            return v(l.weight), _b(l.bias, dev)
+
+        w.img_w, w.img_b = lin(m.img_in)
+        w.txt_norm_w, w.txt_norm_eps = _b(m.txt_norm.weight, dev), m.txt_norm.eps
+        w.txt_w, w.txt_b = lin(m.txt_in)
+        te = m.time_text_embed.timestep_embedder
+        w.t_mlp = (*lin(te.linear_1), *lin(te.linear_2))
+        parts, ada_b, off = [], [], 0
+
+        def ada(l):
+            nonlocal off
+            parts.append((off, v(l.weight)))
+            ada_b.append(l.bias.detach())
+            start, off = off, off + l.weight.shape[0]
+            return start
+
+        for blk in m.transformer_blocks:
+            a = blk.attn
+            d = {"ada": ada(blk.img_mod[1]), "ada_c": ada(blk.txt_mod[1])}
+            for key, q, k, vv, o, nq, nk, mlp in (("", a.to_q, a.to_k, a.to_v, a.to_out[0], a.norm_q, a.norm_k, blk.img_mlp),
+                                                  ("c", a.add_q_proj, a.add_k_proj, a.add_v_proj, a.to_add_out, a.norm_added_q,
+                                                   a.norm_added_k, blk.txt_mlp)):
+                d.update({f"{key}qk_w": (v(q.weight), v(k.weight)), f"{key}qk_b": _b(torch.cat([q.bias, k.bias]), dev),
+                          f"{key}v_w": v(vv.weight), f"{key}v_b": _b(vv.bias, dev), f"{key}o_w": v(o.weight), f"{key}o_b": _b(o.bias, dev),
+                          f"{key}nq": _b(nq.weight, dev), f"{key}nk": _b(nk.weight, dev),
+                          f"{key}ff1_w": v(mlp.net[0].proj.weight), f"{key}ff1_b": _b(mlp.net[0].proj.bias, dev),
+                          f"{key}ff2_w": v(mlp.net[2].weight), f"{key}ff2_b": _b(mlp.net[2].bias, dev)})
+            w.double.append(d)
+        w.ada_out = ada(m.norm_out.linear)
+        w.ada_parts, w.ada_b, w.ada_rows = parts, _b(torch.cat(ada_b), dev), off
+        w.out_w, w.out_b = lin(m.proj_out)
+        w.device = dev
+        return w
+
+
+def qwen_img_shapes(img_shapes):
+    """The image grids of a call as `QwenEmbedRope.forward` reads `img_shapes`: [(1, h, w)] (T2I) and [[(1, h, w), (1, h', w')]]
+    (Edit: the noised latents, then the reference image) both give a tuple of (frames, height, width) per image."""
+    fhw = img_shapes
+    if isinstance(fhw, list):
+        fhw = fhw[0]
+    if not isinstance(fhw, list):
+        fhw = [fhw]
+    return tuple(tuple(int(x) for x in s) for s in fhw)
+
+
+def qwen_rope_positions(shapes, n_txt):
+    """(frame, height, width) position of every row of the joint sequence [txt | img] (diffusers `QwenEmbedRope`, scale_rope=True):
+    image i takes frames i .. i+f-1, row r of an image of height h sits at r - (h - h//2) (centred; the width alike), and text
+    token j at m + j on all three axes, m the largest h//2 or w//2 over the images. int64 [n_txt + sum f*h*w, 3]."""
+    rows, m = [], 0
+    for i, (f, h, w) in enumerate(shapes):
+        fr = torch.arange(i, i + f)
+        hr = torch.arange(h) - (h - h // 2)
+        wr = torch.arange(w) - (w - w // 2)
+        rows.append(torch.stack(torch.meshgrid(fr, hr, wr, indexing="ij"), dim=-1).reshape(-1, 3))
+        m = max(m, h // 2, w // 2)
+    txt = (m + torch.arange(n_txt))[:, None].expand(n_txt, 3)
+    return torch.cat([txt] + rows, dim=0)
+
+
+def qwen_rope_table(shapes, n_txt, device, axes_dim=(16, 56, 56), theta=10000):
+    """cos / sin of `QwenEmbedRope` for the joint sequence [txt | img], [S, 128] fp32 as interleaved (cos, sin) pairs. Upstream
+    forms each angle in fp32 (`torch.outer(index, 1 / theta ** (arange(0, d, 2) / d))`, then `torch.polar`); the same fp32
+    angles are formed here and their cos / sin taken in float64, then rounded to fp32 — within one fp32 ulp of upstream's. This is
+    not FLUX's `rope_table`, whose angles are float64."""
+    pos = qwen_rope_positions(shapes, n_txt)
+    ang = []
+    for i, d in enumerate(axes_dim):
+        inv = 1.0 / torch.pow(theta, torch.arange(0, d, 2).to(torch.float32).div(d))
+        ang.append(torch.outer(pos[:, i].float(), inv))
+    ang = torch.cat(ang, dim=1).double()  # [S, 64], fp32 values
+    cs = torch.stack([ang.cos(), ang.sin()], dim=-1).reshape(len(pos), 128)
+    return cs.float().to(device)
+
+
+class QwenImageEngine(MMDiTCore):
+    """The MMDiT block stack with Qwen-Image's prologue and head, and the per-CFG-branch state of its MagCache forward
+    (MagCache4QwenImage/magcache_generate.py:173-252): the cond and the uncond call of a step have their own text length, so the
+    engine keeps a workspace (and RoPE table) for each of the two most recent (image tokens, text tokens) shapes and one residual
+    slot per branch (`residual_cache[cnt % 2]`), shared by the workspaces. After the first two calls of a generation nothing is
+    allocated but each call's output.
+
+    A hit (`hidden_states += residual_x`, then norm_out / proj_out, :221-247) runs img_in, the time MLP, the final layer's
+    modulation rows, the add, LN+modulate and proj_out: it reads neither the block modulation weights nor the text path."""
+
+    txt_first = True
+    _WS = ("n_img_total", "n_txt", "shard", "n_img", "S", "S_keys", "txt", "img", "txt_g", "img_g", "hs", "h", "att", "x0", "hit",
+           "qk", "v", "cat", "ada", "adaf", "s_hidden", "s_enc", "s_t", "_rope", "_rope_shapes")
+
+    def __init__(self, weights: QwenImageWeights):
+        self.w, self.device = weights, weights.device
+        self.world = 1
+        self._spaces = {}       # (n_img, n_txt) -> workspace attributes, most recently used last
+        self._shape = None
+        self.res, self.spare, self.res_valid = None, None, [False, False]
+        self._masks = []        # InputKeys of the last text masks found all ones
+
+    def _workspace(self, n_img, n_txt):
+        key = (n_img, n_txt)
+        if self._shape == key:
+            return
+        if self.res is None or self.res[0].shape[0] != n_img:  # the residual slots: one per CFG branch, for every text length
+            D = self.w.dim
+            self.res = [torch.empty(n_img, D, dtype=torch.bfloat16, device=self.device) for _ in range(2)]
+            self.spare = torch.empty_like(self.res[0])  # the calibration twin's new residual, swapped into its slot
+            self.res_valid = [False, False]
+        ws = self._spaces.pop(key, None)
+        if ws is None:
+            while len(self._spaces) >= 2:
+                self._spaces.pop(next(iter(self._spaces)))
+            slots, valid = self.res, self.res_valid
+            self._alloc_core(n_img, n_txt)
+            self.res, self.res_valid = slots, valid  # (`_alloc_core`'s single residual buffer is not used)
+            bf = dict(dtype=torch.bfloat16, device=self.device)
+            self.s_hidden = torch.empty(n_img, self.w.in_channels, **bf)
+            self.s_enc = torch.empty(n_txt, self.w.joint_dim, **bf)
+            self.s_t = torch.empty(1, dtype=torch.float64, device=self.device)
+            self._rope, self._rope_shapes = None, None
+            ws = {k: getattr(self, k) for k in self._WS}
+        self._spaces[key] = ws
+        self.__dict__.update(ws)
+        self._shape = key
+
+    def _rope_for(self, rows):
+        return self._rope[rows]
+
+    def stage_inputs(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens):
+        """Checks and stages one call's inputs (one sample). Raises ValueError for `txt_seq_lens` other than [text tokens] and for
+        image grids that do not add up to the image tokens; NotImplementedError for more than one sample and for a text mask with
+        zeros (upstream's attention ignores the mask: its pipeline trims the prompt to the valid tokens of a one-prompt batch)."""
+        if hidden_states.dim() != 3 or hidden_states.shape[0] != 1 or encoder_hidden_states.shape[0] != 1 or timestep.numel() != 1:
+            raise NotImplementedError("magcache_b200: the Qwen-Image engine runs one sample per call (true CFG as two calls)")
+        n_img, n_txt = hidden_states.shape[1], encoder_hidden_states.shape[1]
+        if txt_seq_lens is None or list(txt_seq_lens) != [n_txt]:
+            raise ValueError(f"magcache_b200: txt_seq_lens must be [{n_txt}] (the text tokens of the call); got {txt_seq_lens}")
+        shapes = qwen_img_shapes(img_shapes)
+        if sum(f * h * w for f, h, w in shapes) != n_img:
+            raise ValueError(f"magcache_b200: img_shapes {list(shapes)} cover {sum(f * h * w for f, h, w in shapes)} tokens, "
+                             f"hidden_states has {n_img}")
+        m = encoder_hidden_states_mask
+        if m is not None and not any(k.matches(m) for k in self._masks):  # one host read per new mask
+            if tuple(m.shape) != (1, n_txt) or not bool((m == 1).all()):
+                raise NotImplementedError("magcache_b200: encoder_hidden_states_mask must be None or all ones [1, text tokens]: "
+                                          "padded prompts are not supported")
+            self._masks = self._masks[-1:] + [InputKey(m)]
+        self._workspace(n_img, n_txt)
+        self.s_hidden.copy_(hidden_states[0])
+        self.s_enc.copy_(encoder_hidden_states[0])
+        # `timestep.to(bf16)` (:195), then Timesteps(256, scale=1000) forms 1000 * t * freq in fp32 [EXT diffusers]; the sinusoid
+        # kernel takes float(bf16(t)) * 1000 and forms its arguments in float64 (finer than upstream's fp32, as for Open-Sora)
+        self.s_t.copy_(timestep.reshape(1).to(torch.bfloat16).double() * 1000)
+        if self._rope_shapes != shapes:
+            self._rope, self._rope_shapes = qwen_rope_table(shapes, n_txt, self.device), shapes
+            self._spaces[self._shape].update(_rope=self._rope, _rope_shapes=shapes)
+
+    def prologue(self, full):
+        """img_in and the time embedding (:194-202); on a miss or a calibration call (`full`) also the modulation table of every
+        block and txt_norm -> txt_in into the text rows. A hit computes only the final layer's two modulation chunks."""
+        w = self.w
+        ops.gemm(self.s_hidden, w.img_w, w.img_b, E.MC_EPI_BIAS_BF16, out=self.x0)
+        temb = self._time_mlp(self._sinusoid(self.s_t), w.t_mlp)
+        if full:
+            self._modulation_table(temb)
+            ops.rmsnorm_rope_(self.s_enc, w.txt_norm_w, None, eps=w.txt_norm_eps)  # RMSNorm(3584): bf16(bf16(x rsqrt(ms + eps)) w)
+            ops.gemm(self.s_enc, w.txt_w, w.txt_b, E.MC_EPI_BIAS_BF16, out=self.hs[self.txt])
+        else:
+            r0, r1 = w.ada_out, w.ada_out + 2 * w.dim
+            ops.gemm(ops.silu(temb), w.ada_parts[-1][1], w.ada_b[r0:r1], E.MC_EPI_BIAS_BF16, out=self.ada[:, r0:r1])
+            ops.cast_into(self.ada.view(-1)[r0:r1], self.adaf[r0:r1])
+        return self.x0
+
+    def head(self, x_img):
+        """`norm_out(hidden_states, temb)` (AdaLayerNormContinuous: scale, shift in that order) and `proj_out` (:246-247)."""
+        w = self.w
+        ops.ln_modulate(x_img, self._em(w.ada_out, 2), 0, 1, round_ln_to_bf16=True, out=self.h[self.img])
+        return ops.gemm(self.h[self.img], w.out_w, w.out_b, E.MC_EPI_BIAS_BF16)
+
+    def forward(self, kind, slot):
+        """hit: `hidden_states += residual_cache[slot]` (:221-222) | miss: the 60 blocks, residual into the slot (:224-239); then the
+        head."""
+        if kind == "hit":
+            if not self.res_valid[slot]:
+                raise TypeError("magcache_b200: cache hit with an empty residual cache (reference: Tensor += NoneType)")
+            x = ops.cache_hit_add(self.prologue(full=False), self.res[slot], out=self.hit)
+        else:
+            x0 = self.prologue(full=True)
+            self.hs[self.img].copy_(x0)
+            x = self.run_blocks()
+            ops.residual_sub(x, x0, out=self.res[slot])
+            self.res_valid[slot] = True
+        return self.head(x)
+
+    def calibrate(self, slot, compare):
+        """The calibration twin (:94-171): the blocks always run; with `compare`, (norm_ratio, norm_std, cos_dis) of the new
+        residual against the slot's (fused fp32/fp64 reduction, finer than upstream's bf16 tensor ops), else None. The new residual
+        then takes the slot."""
+        x0 = self.prologue(full=True)
+        self.hs[self.img].copy_(x0)
+        x = self.run_blocks()
+        new = self.spare
+        ops.residual_sub(x, x0, out=new)
+        stats = None
+        if compare:
+            if not self.res_valid[slot]:
+                raise TypeError("magcache_b200: calibration statistics against an empty residual slot (reference: NoneType.norm)")
+            stats = ops.residual_stats(new, self.res[slot])
+        self.res[slot], self.spare = new, self.res[slot]
+        self.res_valid[slot] = True
+        return self.head(x), stats
+
+
+# ======================================================================================================================
 # Synthetic weights created directly on the device (benchmarks: a FLUX.1-dev / HunyuanVideo-sized nn.Module does not fit a CPU box)
 # ======================================================================================================================
 def _rand_block_weights(D, dev, g, keys_prefix=("", "c")):
@@ -1068,6 +1325,34 @@ def random_hunyuan_weights(dev, heads=24, double_depth=20, single_depth=40, in_c
                           "o_w": xav(D, D), "o_b": bias(D), "f1_w": xav(4 * D, D), "f1_b": bias(4 * D), "f2_w": xav(D, 4 * D), "f2_b": bias(D)})
     w.r_ada_w, w.r_ada_b = xav(4 * D, D, 0.3), bias(4 * D)
     w.out_w, w.out_b = xav(in_channels * 4, D), bias(in_channels * 4)
+    return w
+
+
+def random_qwen_weights(dev, heads=24, num_layers=60, in_channels=64, out_channels=16, joint_dim=3584, seed=0):
+    """QwenImageWeights of the Qwen-Image shape on synthetic device weights, one tensor per Linear like a loaded module's."""
+    g = torch.Generator(device=dev).manual_seed(seed)
+    w = QwenImageWeights()
+    w.heads, w.dim = heads, heads * 128
+    D = w.dim
+    w.in_channels, w.joint_dim, w.device, w.txt_norm_eps = in_channels, joint_dim, dev, 1e-6
+    d, xav, bias, nw = _rand_block_weights(D, dev, g)
+    parts, off = [], 0
+    for _ in range(num_layers):
+        d, *_ = _rand_block_weights(D, dev, g)
+        for k in ("", "c"):
+            q, kk = d[f"{k}qk_w"].split(D)
+            d[f"{k}qk_w"] = (q.contiguous(), kk.contiguous())
+        d["ada"], d["ada_c"] = off, off + 6 * D
+        parts += [(off, xav(6 * D, D, 0.3)), (off + 6 * D, xav(6 * D, D, 0.3))]
+        off += 12 * D
+        w.double.append(d)
+    w.ada_out = off
+    parts.append((off, xav(2 * D, D, 0.3)))
+    w.ada_parts, w.ada_b, w.ada_rows = parts, bias(off + 2 * D), off + 2 * D
+    w.img_w, w.img_b, w.txt_w, w.txt_b = xav(D, in_channels), bias(D), xav(D, joint_dim), bias(D)
+    w.txt_norm_w = (1 + 0.1 * torch.randn(joint_dim, device=dev, generator=g)).bfloat16().float()
+    w.t_mlp = (xav(D, 256), bias(D), xav(D, D), bias(D))
+    w.out_w, w.out_b = xav(4 * out_channels, D), bias(4 * out_channels)
     return w
 
 

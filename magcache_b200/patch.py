@@ -21,14 +21,14 @@ import torch
 
 from . import ops
 from .config import FAMILIES, interp_cfg, nearest_interp, save_json, table_for_ckpt_dir, table_from_calibration, tables
-from .controller import AttrController, OpenSoraTeaController, TeaController, opensora_rel_l1
+from .controller import AttrController, OpenSoraTeaController, TeaController, nearest_interp_linspace, opensora_rel_l1
 from .lora import is_lora_layer, scale_lora_layers, unscale_lora_layers
-from .mmdit import FluxEngine, FluxWeights, HunyuanEngine, HunyuanWeights
+from .mmdit import FluxEngine, FluxWeights, HunyuanEngine, HunyuanWeights, QwenImageEngine, QwenImageWeights
 from .opensora import OpenSoraEngine, OpenSoraWeights
 from .wan import WanEngine, WanWeights
 
 # every engine a patched forward caches on its module (one per model family)
-ENGINE_ATTRS = ("_mc_engine", "_mc_flux_engine", "_mc_hunyuan_engine", "_mc_opensora_engine")
+ENGINE_ATTRS = ("_mc_engine", "_mc_flux_engine", "_mc_hunyuan_engine", "_mc_opensora_engine", "_mc_qwen_engine")
 
 
 def _cached_engine(self, attr, build):
@@ -578,6 +578,108 @@ def init_magcache_hunyuan(transformer, infer_steps=50, thresh=0.24, K=6, retenti
     cls.forward = magcache_hunyuan_forward
     cls.accumulated_ratio, cls.accumulated_err, cls.accumulated_steps = 1, 0, 0
     return transformer
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Qwen-Image / Qwen-Image-Edit (MagCache4QwenImage/magcache_generate.py, MagCache4QwenImageEdit/magcache_generate.py: the same
+# forward, calibration and installation statements) on the MMDiT engine
+# ------------------------------------------------------------------------------------------------------------------
+def _qwen_stage(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens, guidance,
+                attention_kwargs):
+    if guidance is not None:
+        raise NotImplementedError("magcache_b200: Qwen-Image guidance (guidance_embeds checkpoints) is not supported")
+    extra = dict(attention_kwargs or {})
+    scale = extra.pop("scale", 1.0)
+    if extra or scale != 1.0:
+        raise NotImplementedError(f"magcache_b200: the Qwen-Image engine takes no attention_kwargs but scale 1.0; got {attention_kwargs}")
+    if self.__dict__.get("_mc_shard_kw", {}).get("shard_world", 1) > 1:
+        raise NotImplementedError("magcache_b200: the Qwen-Image engine has no token-sharded path; run it on one GPU")
+    if not hidden_states.is_cuda:
+        raise RuntimeError("magcache_b200: hidden_states must be CUDA tensors (no CPU path)")
+    eng = _cached_engine(self, "_mc_qwen_engine", lambda **kw: QwenImageEngine(QwenImageWeights.from_module(self, hidden_states.device)))
+    eng.stage_inputs(hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens)
+    return eng
+
+
+def magcache_qwen_image_forward(self, hidden_states, encoder_hidden_states=None, encoder_hidden_states_mask=None, timestep=None,
+                                img_shapes=None, txt_seq_lens=None, guidance=None, attention_kwargs=None, return_dict=True):
+    r"""MagCache4QwenImage/magcache_generate.py:173-252 (Qwen-Image-Edit: the same lines of its script) on the H100 kernels: same
+    signature and state attributes (`cnt, num_steps, magcache_thresh, K, retention_ratio, accumulated_ratio / _err / _steps` as
+    per-branch lists, `residual_cache` indexed by `cnt % 2`, `mag_ratios`), `(output,)` or an object with `.sample`. One sample per
+    call: the pipelines' true CFG makes a cond and an uncond call per step, each with its own text length and residual slot. A
+    hit runs only img_in, the time embedding, the add and the final layer (mmdit.QwenImageEngine)."""
+    eng = _qwen_stage(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens,
+                      guidance, attention_kwargs)
+    slot = int(self.cnt) % 2
+    skip_forward = _ctrl(self, "qwen-image").decide(self)  # :205-219
+    _take_residual(eng, self.residual_cache[slot], slot)
+    out = eng.forward("hit" if skip_forward else "miss", slot)
+    self.residual_cache[slot] = eng.res[slot].view(1, *eng.res[slot].shape)  # :241
+    self.cnt += 1  # :242-244, the reference's own statements: the wrap rebinds an int on the instance and keeps the accumulators
+    if self.cnt >= self.num_steps:
+        self.cnt = 0
+    output = out.view(1, *out.shape)
+    return _Sample(output) if return_dict else (output,)
+
+
+def magcache_qwen_image_calibration(self, hidden_states, encoder_hidden_states=None, encoder_hidden_states_mask=None, timestep=None,
+                                    img_shapes=None, txt_seq_lens=None, guidance=None, attention_kwargs=None, return_dict=True):
+    r"""MagCache4QwenImage/magcache_generate.py:94-171: every call runs the blocks; from `cnt >= 2` on the residual is compared with
+    the one of the same CFG branch (`residual_cache[cnt % 2]`) and `norm_ratio / norm_std / cos_dis` get one entry each (rounded to 5
+    places), printed per step in the reference's format. At the wrap the lists are printed and only the counter is reset."""
+    eng = _qwen_stage(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens,
+                      guidance, attention_kwargs)
+    slot = int(self.cnt) % 2
+    _take_residual(eng, self.residual_cache[slot], slot)
+    out, stats = eng.calibrate(slot, compare=self.cnt >= 2)
+    if stats is not None:  # :143-153
+        norm_ratio, norm_std, cos_dis = stats
+        self.norm_ratio.append(round(norm_ratio, 5))
+        self.norm_std.append(round(norm_std, 5))
+        self.cos_dis.append(round(cos_dis, 5))
+        print(f"Step {self.cnt}: norm_ratio={norm_ratio:.5f}, norm_std={norm_std:.5f}, cos_dis={cos_dis:.5f}")
+    self.residual_cache[slot] = eng.res[slot].view(1, *eng.res[slot].shape)  # :155
+    self.cnt += 1
+    if self.cnt >= self.num_steps:  # :158-163
+        self.cnt = 0
+        print("\nCalibration Results:")
+        print("norm_ratio:", self.norm_ratio)
+        print("norm_std:", self.norm_std)
+        print("cos_dis:", self.cos_dis)
+    output = out.view(1, *out.shape)
+    return _Sample(output) if return_dict else (output,)
+
+
+def init_magcache_qwen_image(model, mag_ratios, sample_steps=50, thresh=0.06, K=2, retention_ratio=0.2):
+    """`init_magcache(model, mag_ratios, args)` of MagCache4QwenImage/magcache_generate.py:63-83 (and the Edit script): patches the
+    CLASS. `mag_ratios`: the list without its `[1.0]*2` prefix as the scripts pass it, or a key of `tables()` ("qwen_image",
+    "qwen_image_edit"), which carries the prefix. A table of another length is resampled per branch by `np.linspace` rounding."""
+    cls = model.__class__
+    cls.forward = magcache_qwen_image_forward
+    cls.cnt = torch.tensor(0)
+    cls.num_steps = sample_steps * 2
+    cls.split_step, cls.mode = None, "t2v"
+    cls.magcache_thresh, cls.K = thresh, K
+    cls.accumulated_err, cls.accumulated_steps, cls.accumulated_ratio = [0.0, 0.0], [0, 0], [1.0, 1.0]
+    cls.retention_ratio = retention_ratio
+    cls.residual_cache = [None, None]
+    mr = tables()[mag_ratios] if isinstance(mag_ratios, str) else np.array([1.0] * 2 + list(mag_ratios))
+    if len(mr) != sample_steps * 2:  # :79-83
+        con, ucon = nearest_interp_linspace(mr[0::2], sample_steps), nearest_interp_linspace(mr[1::2], sample_steps)
+        mr = np.concatenate([con.reshape(-1, 1), ucon.reshape(-1, 1)], axis=1).flatten()
+    cls.mag_ratios = mr
+    return model
+
+
+def init_magcache_qwen_image_calibration(model, sample_steps=50):
+    """`init_magcache_calibration(model, args)` of MagCache4QwenImage/magcache_generate.py:85-92."""
+    cls = model.__class__
+    cls.forward = magcache_qwen_image_calibration
+    cls.cnt = torch.tensor(0)
+    cls.num_steps = sample_steps * 2
+    cls.norm_ratio, cls.norm_std, cls.cos_dis = [], [], []
+    cls.residual_cache = [None, None]
+    return model
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -6,6 +6,7 @@ usage (GPU): python tools/bench_mmdit.py flux|hunyuan [--steps N] [--no-cache] [
              python tools/bench_mmdit.py flux --controlnet D,S [--controlnet-repeat] [--rounds R] [--steps N]
              python tools/bench_mmdit.py flux --lora RANK [--rounds R] [--steps N]
              python tools/bench_mmdit.py flux --ip-adapter A[,T] [--rounds R] [--steps N]
+             python tools/bench_mmdit.py qwen-image [--edit] [--rounds R] [--steps N]
 
 --controlnet D,S: the FLUX 1024^2 miss forward (the whole block stack) with D double-block and S single-block synthetic bf16
 ControlNet samples (S = 0: none for the single blocks) against the same forward without samples, timed in alternating rounds of N
@@ -17,7 +18,12 @@ without adapters, alternating rounds as for --controlnet.
 
 --ip-adapter A[,T]: the FLUX 1024^2 miss and hit forwards with A synthetic XLabs-shaped IP-Adapters (768-wide image embeds projected
 to T tokens of 4096, default T = 16; `to_k_ip` / `to_v_ip` on all 19 double blocks) against the same forwards without them,
-alternating rounds as for --controlnet; then `mc_ip_attn` alone at 4096 rows with its bytes per launch and rate."""
+alternating rounds as for --controlnet; then `mc_ip_attn` alone at 4096 rows with its bytes per launch and rate.
+
+qwen-image: Qwen-Image (60 blocks, 3072 wide, synthetic weights) at 1328^2 (6889 image tokens; --edit: Qwen-Image-Edit's 1024^2
+noised latents plus a 1024^2 reference image, 8192 tokens) with a 200-token cond and a 6-token uncond prompt: cond miss, uncond
+miss and hit medians (CUDA events, alternating rounds of N forwards), peak memory, and the 50-step transformer time of the
+qwen-image-E006K2R02 schedule from those medians."""
 import argparse
 import json
 import os
@@ -209,9 +215,45 @@ def bench_ip_adapter(n_adapters, T, rounds, per_round):
                       "rounds": rounds, "forwards_per_round": per_round, "gpu": name, "power_limit": power}))
 
 
+def bench_qwen_image(edit, rounds, per_round):
+    dev = torch.device("cuda:0")
+    g = torch.Generator(device=dev).manual_seed(0)
+    torch.cuda.reset_peak_memory_stats()
+    eng = mmdit.QwenImageEngine(mmdit.random_qwen_weights(dev))
+    weights = torch.cuda.memory_allocated()
+    shapes = [[(1, 64, 64), (1, 64, 64)]] if edit else [(1, 83, 83)]
+    n_img = 8192 if edit else 6889
+    hs = torch.randn(1, n_img, 64, device=dev, generator=g).bfloat16()
+    enc = {n: torch.randn(1, n, 3584, device=dev, generator=g).bfloat16() for n in (200, 6)}
+    t = torch.tensor([0.6], device=dev)
+    slot = {200: 0, 6: 1}
+    modes = {n: (lambda n=n: eng.stage_inputs(hs, enc[n], None, t, shapes, [n])) for n in enc}
+
+    class Slotted:  # `_alternate` calls forward(kind); the slot follows the branch
+        def __init__(self):
+            self.n = 200
+
+        def forward(self, kind):
+            return eng.forward(kind, slot[self.n])
+
+    sl = Slotted()
+    modes = {n: (lambda n=n, f=f: (setattr(sl, "n", n), f())) for n, f in modes.items()}
+    times = _alternate(sl, modes, ("miss", "hit"), rounds, per_round)
+    med = {k: statistics.median(v) for k, v in times.items()}
+    mask = mc.PRESETS["qwen-image-edit-E006K2R02" if edit else "qwen-image-E006K2R02"].schedule()
+    total = sum(med[(200 if i % 2 == 0 else 6, "hit" if s else "miss")] for i, s in enumerate(mask))
+    name, power = card()
+    print(json.dumps({"family": "qwen-image-edit" if edit else "qwen-image", "gpu": name, "power_limit": power, "image_tokens": n_img,
+                      "miss_cond_ms": med[(200, "miss")], "miss_uncond_ms": med[(6, "miss")], "hit_ms": med[(200, "hit")],
+                      "spread_ms": {f"{k[0]}_{k[1]}": [min(v), max(v)] for k, v in times.items()},
+                      "peak_gib": torch.cuda.max_memory_allocated() / 2**30, "engine_weights_gib": weights / 2**30,
+                      "E006K2R02_50_steps_s": total / 1e3, "hits": int(sum(mask)), "calls": len(mask)}))
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("family", choices=["flux", "hunyuan"])
+    ap.add_argument("family", choices=["flux", "hunyuan", "qwen-image"])
+    ap.add_argument("--edit", action="store_true", help="qwen-image: Qwen-Image-Edit's two 1024^2 images")
     ap.add_argument("--steps", type=int, default=None)
     ap.add_argument("--no-cache", action="store_true")
     ap.add_argument("--frames", type=int, default=33, help="hunyuan: latent frames (33 = 129 video frames)")
@@ -221,6 +263,9 @@ def main():
     ap.add_argument("--ip-adapter", default=None, help="flux: A[,T] IP-Adapters of T image-prompt tokens (default 16); times miss and hit forwards with and without")
     ap.add_argument("--rounds", type=int, default=5, help="--controlnet / --lora / --ip-adapter: alternating rounds")
     args = ap.parse_args()
+    if args.family == "qwen-image":
+        bench_qwen_image(args.edit, args.rounds, args.steps or 3)
+        return
     if args.ip_adapter is not None:
         if args.family != "flux":
             ap.error("--ip-adapter is a FLUX option")
