@@ -28,7 +28,7 @@ import numpy as np
 import torch
 
 from . import _lib, ops
-from .lora import FluxLoraScan, LoraPack, Tailed, base_linear, is_lora_layer
+from .lora import FLUX as FLUX_LORA, QWEN as QWEN_LORA, LoraPack, LoraScan, Tailed, base_linear, is_lora_layer
 from .ops import IP_ATTN_MAX_ADAPTERS, IP_ATTN_MAX_KEYS
 
 E = _lib
@@ -324,8 +324,28 @@ class MMDiTCore:
     ada_w / ada_b / ada_rows), the token order (`txt_first`), the RoPE table of the rows that get RoPE, and its own prologue / head."""
 
     txt_first = True
-    lora = None  # lora.LoraPack of the current call (FLUX with unmerged adapters), else None
+    lora = None  # lora.LoraPack of the current call (FLUX / Qwen-Image with unmerged adapters), else None
     ip = None    # IPAdapterCall of the current call (FLUX with IP-Adapter processors), else None
+    lora_family = None  # lora.FLUX / lora.QWEN: where the family's adapters may sit and where they pack
+    _lora_scan, _lora_merged, _lora_wrappers = None, (), ()
+
+    def sync_lora(self, module):
+        """Take the module's unmerged LoRA adapters as they are now (lora.LoraScan): called at every forward and calibration call,
+        after the reference's `scale_lora_layers`. Base weights are reread from the module when a merge or unmerge happened since
+        they were read, and when a LoRA layer seen before has left the module (it may have been merged first: `fuse_lora()` then
+        `unload_lora_weights()`); otherwise only what changed is repacked (lora.LoraPack)."""
+        first = self._lora_scan is None
+        if first:
+            self._lora_scan = LoraScan(module, self.lora_family)
+        spec, merged, wrappers, changed = self._lora_scan.scan()
+        now = {id(m) for m in wrappers}
+        if not first and (merged != self._lora_merged or any(id(m) not in now for m in self._lora_wrappers)):
+            self.w = type(self.w).from_module(module, self.device)
+            self.lora, changed = None, True
+        # the layers themselves are kept (not their ids), so an id cannot be reused by a new layer before the next comparison
+        self._lora_merged, self._lora_wrappers = merged, wrappers
+        if changed:
+            self.lora = LoraPack(self.w, spec, self.lora, self.lora_family) if spec else None
 
     def _controlnet_views(self):
         """`run_blocks`' ControlNet argument for the current call; only the FLUX engine takes ControlNet residuals."""
@@ -389,7 +409,8 @@ class MMDiTCore:
             ops.gemm(ops.silu(vec), w.ada_w, w.ada_b, E.MC_EPI_BIAS_BF16, out=self.ada)
         else:  # FP8 block rows and bf16 final-layer rows, or LoRA-adapted rows apart from the others: each output column still
             s = ops.silu(vec)  # comes from its own row of the stack
-            self._down(self.lora.groups if self.lora is not None else {}, "ada", s)
+            for g in ("ada", "ada_out"):
+                self._down(self.lora.groups if self.lora is not None else {}, g, s)
             for r0, wt in parts:
                 r1 = r0 + wt.shape[0]
                 self._linear(s, wt, w.ada_b[r0:r1], E.MC_EPI_BIAS_BF16, out=self.ada[:, r0:r1])
@@ -592,6 +613,7 @@ class MMDiTCore:
 
 class FluxEngine(MMDiTCore):
     txt_first = True
+    lora_family = FLUX_LORA
 
     def __init__(self, weights: FluxWeights, shard_world=1, shard_rank=0, shard_group=None):
         self.w, self.device = weights, weights.device
@@ -602,24 +624,6 @@ class FluxEngine(MMDiTCore):
         self.controlnet = (None, None, False)
         self._lora_scan, self._lora_merged, self._lora_wrappers = None, (), ()
         self.ip = None
-
-    def sync_lora(self, module):
-        """Take the module's unmerged LoRA adapters as they are now (lora.FluxLoraScan): called at every forward, after the
-        reference's `scale_lora_layers`. Base weights are repacked from the module when a merge or unmerge happened since they
-        were packed, and when a LoRA layer seen before has left the module (it may have been merged first: `fuse_lora()` then
-        `unload_lora_weights()`); otherwise only what changed is repacked (lora.LoraPack)."""
-        first = self._lora_scan is None
-        if first:
-            self._lora_scan = FluxLoraScan(module)
-        spec, merged, wrappers, changed = self._lora_scan.scan()
-        now = {id(m) for m in wrappers}
-        if not first and (merged != self._lora_merged or any(id(m) not in now for m in self._lora_wrappers)):
-            self.w = FluxWeights.from_module(module, self.device)
-            self.lora, changed = None, True
-        # the layers themselves are kept (not their ids), so an id cannot be reused by a new layer before the next comparison
-        self._lora_merged, self._lora_wrappers = merged, wrappers
-        if changed:
-            self.lora = LoraPack(self.w, spec, self.lora) if spec else None
 
     def _workspace(self, n_img, n_txt):
         if self._shape == (n_img, n_txt):
@@ -1006,7 +1010,12 @@ class QwenImageWeights:
     At 20 B parameters (40.9 GB in bf16) nothing large is copied: every block matrix is the module's own bf16 weight, read in
     place. The modulation rows stay one part per Linear (`ada_parts`; a stacked copy would be 13.6 GB), and q and k run as two
     GEMMs into the halves of `qk` instead of one over a fused q|k copy (4.5 GB): 240 more GEMM launches per miss, each over half
-    the columns. The engine's own copies are the biases and norm weights, as fp32 (22 MB at full size)."""
+    the columns. The engine's own copies are the biases and norm weights, as fp32 (22 MB at full size).
+
+    Base weights only: a PEFT LoRA layer contributes its `base_layer`, read in place like any other Linear; the adapters are read
+    at every call (lora.py, `MMDiTCore.sync_lora`). An in-place merge is therefore already in the weights read here, but PEFT's
+    `safe_merge=True` rebinds `weight.data` to a new tensor, so `sync_lora` rereads them on every merge or unmerge it sees (cheap:
+    only the fp32 biases and norm weights are copied)."""
 
     fp8_scratch = None
 
@@ -1015,17 +1024,15 @@ class QwenImageWeights:
 
     @classmethod
     def from_module(cls, m, dev):
-        for name, mod in m.named_modules():
-            if is_lora_layer(mod):
-                raise NotImplementedError(f"magcache_b200: the Qwen-Image engine runs no LoRA adapters; {name} carries one "
-                                          "(merge it into the weights first)")
         cfg = m.config
         if cfg.attention_head_dim != 128 or tuple(cfg.axes_dims_rope) != (16, 56, 56):
             raise NotImplementedError("magcache_b200: the Qwen-Image engine needs head_dim 128 with RoPE axes (16, 56, 56)")
         if getattr(cfg, "guidance_embeds", False):
             raise NotImplementedError("magcache_b200: Qwen-Image with guidance_embeds is not supported (the released checkpoints have none)")
+        adapter = {id(p) for mod in m.modules() if is_lora_layer(mod)  # (LoraPack converts adapter weights itself)
+                   for n, p in mod.named_parameters() if not n.startswith("base_layer.")}
         for name, p in m.named_parameters():
-            if p.dtype != torch.bfloat16 or p.device != dev:
+            if id(p) not in adapter and (p.dtype != torch.bfloat16 or p.device != dev):
                 raise NotImplementedError(f"magcache_b200: the Qwen-Image engine reads the module's bf16 weights in place on {dev}; "
                                           f"{name} is {p.dtype} on {p.device}")
         w = cls()
@@ -1033,9 +1040,10 @@ class QwenImageWeights:
         w.dim = D = w.heads * 128
         w.in_channels, w.joint_dim = cfg.in_channels, cfg.joint_attention_dim
         v = lambda t: t.detach()  # noqa: E731  (the module's own storage)
+        B = base_linear
 
         def lin(l):
-            return v(l.weight), _b(l.bias, dev)
+            return v(B(l).weight), _b(B(l).bias, dev)
 
         w.img_w, w.img_b = lin(m.img_in)
         w.txt_norm_w, w.txt_norm_eps = _b(m.txt_norm.weight, dev), m.txt_norm.eps
@@ -1046,6 +1054,7 @@ class QwenImageWeights:
 
         def ada(l):
             nonlocal off
+            l = B(l)
             parts.append((off, v(l.weight)))
             ada_b.append(l.bias.detach())
             start, off = off, off + l.weight.shape[0]
@@ -1057,11 +1066,12 @@ class QwenImageWeights:
             for key, q, k, vv, o, nq, nk, mlp in (("", a.to_q, a.to_k, a.to_v, a.to_out[0], a.norm_q, a.norm_k, blk.img_mlp),
                                                   ("c", a.add_q_proj, a.add_k_proj, a.add_v_proj, a.to_add_out, a.norm_added_q,
                                                    a.norm_added_k, blk.txt_mlp)):
+                q, k, vv, o, f1, f2 = (B(x) for x in (q, k, vv, o, mlp.net[0].proj, mlp.net[2]))
                 d.update({f"{key}qk_w": (v(q.weight), v(k.weight)), f"{key}qk_b": _b(torch.cat([q.bias, k.bias]), dev),
                           f"{key}v_w": v(vv.weight), f"{key}v_b": _b(vv.bias, dev), f"{key}o_w": v(o.weight), f"{key}o_b": _b(o.bias, dev),
                           f"{key}nq": _b(nq.weight, dev), f"{key}nk": _b(nk.weight, dev),
-                          f"{key}ff1_w": v(mlp.net[0].proj.weight), f"{key}ff1_b": _b(mlp.net[0].proj.bias, dev),
-                          f"{key}ff2_w": v(mlp.net[2].weight), f"{key}ff2_b": _b(mlp.net[2].bias, dev)})
+                          f"{key}ff1_w": v(f1.weight), f"{key}ff1_b": _b(f1.bias, dev),
+                          f"{key}ff2_w": v(f2.weight), f"{key}ff2_b": _b(f2.bias, dev)})
             w.double.append(d)
         w.ada_out = ada(m.norm_out.linear)
         w.ada_parts, w.ada_b, w.ada_rows = parts, _b(torch.cat(ada_b), dev), off
@@ -1119,11 +1129,13 @@ class QwenImageEngine(MMDiTCore):
     allocated but each call's output.
 
     A hit (`hidden_states += residual_x`, then norm_out / proj_out, :221-247) runs img_in, the time MLP, the final layer's
-    modulation rows, the add, LN+modulate and proj_out: it reads neither the block modulation weights nor the text path."""
+    modulation rows, the add, LN+modulate and proj_out: it reads neither the block modulation weights nor the text path, and with
+    unmerged LoRA adapters only those of img_in, norm_out.linear and proj_out (their own down-projection groups, lora.QWEN)."""
 
     txt_first = True
+    lora_family = QWEN_LORA
     _WS = ("n_img_total", "n_txt", "shard", "n_img", "S", "S_keys", "txt", "img", "txt_g", "img_g", "hs", "h", "att", "x0", "hit",
-           "qk", "v", "cat", "ada", "adaf", "s_hidden", "s_enc", "s_t", "_rope", "_rope_shapes")
+           "qk", "v", "cat", "ada", "adaf", "s_hidden", "s_enc", "s_t", "_rope", "_rope_shapes", "_lora_u")
 
     def __init__(self, weights: QwenImageWeights):
         self.w, self.device = weights, weights.device
@@ -1154,6 +1166,7 @@ class QwenImageEngine(MMDiTCore):
             self.s_enc = torch.empty(n_txt, self.w.joint_dim, **bf)
             self.s_t = torch.empty(1, dtype=torch.float64, device=self.device)
             self._rope, self._rope_shapes = None, None
+            self._lora_u = {}
             ws = {k: getattr(self, k) for k in self._WS}
         self._spaces[key] = ws
         self.__dict__.update(ws)
@@ -1161,6 +1174,19 @@ class QwenImageEngine(MMDiTCore):
 
     def _rope_for(self, rows):
         return self._rope[rows]
+
+    def _down(self, groups, key, x):
+        """`MMDiTCore._down` into this workspace's U buffer of (input, rows, padded rank): the cond and uncond calls of a step share
+        one pack but have their own text rows. Every U is read by the GEMMs right after its down-projection, so all blocks share
+        the buffer; after a workspace's first call with adapters nothing more is allocated."""
+        g = groups.get(key)
+        if g is None:
+            return
+        k = (key, x.shape[0], g.A.shape[0])
+        u = self._lora_u.get(k)
+        if u is None:
+            u = self._lora_u[k] = torch.empty(x.shape[0], g.A.shape[0], dtype=torch.bfloat16, device=self.device)
+        g.u, g.src = ops.gemm(x, g.A, out=u), x
 
     def stage_inputs(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens):
         """Checks and stages one call's inputs (one sample). Raises ValueError for `txt_seq_lens` other than [text tokens] and for
@@ -1193,17 +1219,25 @@ class QwenImageEngine(MMDiTCore):
 
     def prologue(self, full):
         """img_in and the time embedding (:194-202); on a miss or a calibration call (`full`) also the modulation table of every
-        block and txt_norm -> txt_in into the text rows. A hit computes only the final layer's two modulation chunks."""
+        block and txt_norm -> txt_in into the text rows. A hit computes only the final layer's two modulation chunks. LoRA
+        adapters (`self.lora`) on img_in, txt_in and the modulation Linears run as tails of these GEMMs."""
         w = self.w
-        ops.gemm(self.s_hidden, w.img_w, w.img_b, E.MC_EPI_BIAS_BF16, out=self.x0)
+        lg = self.lora.groups if self.lora is not None else {}
+        top = self.lora.top if self.lora is not None else {"img_w": w.img_w, "txt_w": w.txt_w}
+        self._down(lg, "x", self.s_hidden)
+        self._linear(self.s_hidden, top["img_w"], w.img_b, E.MC_EPI_BIAS_BF16, out=self.x0)
         temb = self._time_mlp(self._sinusoid(self.s_t), w.t_mlp)
         if full:
             self._modulation_table(temb)
             ops.rmsnorm_rope_(self.s_enc, w.txt_norm_w, None, eps=w.txt_norm_eps)  # RMSNorm(3584): bf16(bf16(x rsqrt(ms + eps)) w)
-            ops.gemm(self.s_enc, w.txt_w, w.txt_b, E.MC_EPI_BIAS_BF16, out=self.hs[self.txt])
+            self._down(lg, "ctx", self.s_enc)
+            self._linear(self.s_enc, top["txt_w"], w.txt_b, E.MC_EPI_BIAS_BF16, out=self.hs[self.txt])
         else:
             r0, r1 = w.ada_out, w.ada_out + 2 * w.dim
-            ops.gemm(ops.silu(temb), w.ada_parts[-1][1], w.ada_b[r0:r1], E.MC_EPI_BIAS_BF16, out=self.ada[:, r0:r1])
+            parts = w.ada_parts if self.lora is None or self.lora.ada_parts is None else self.lora.ada_parts
+            s = ops.silu(temb)
+            self._down(lg, "ada_out", s)
+            self._linear(s, parts[-1][1], w.ada_b[r0:r1], E.MC_EPI_BIAS_BF16, out=self.ada[:, r0:r1])
             ops.cast_into(self.ada.view(-1)[r0:r1], self.adaf[r0:r1])
         return self.x0
 
@@ -1211,7 +1245,10 @@ class QwenImageEngine(MMDiTCore):
         """`norm_out(hidden_states, temb)` (AdaLayerNormContinuous: scale, shift in that order) and `proj_out` (:246-247)."""
         w = self.w
         ops.ln_modulate(x_img, self._em(w.ada_out, 2), 0, 1, round_ln_to_bf16=True, out=self.h[self.img])
-        return ops.gemm(self.h[self.img], w.out_w, w.out_b, E.MC_EPI_BIAS_BF16)
+        if self.lora is None:
+            return ops.gemm(self.h[self.img], w.out_w, w.out_b, E.MC_EPI_BIAS_BF16)
+        self._down(self.lora.groups, "head", self.h[self.img])
+        return self._linear(self.h[self.img], self.lora.top["out_w"], w.out_b, E.MC_EPI_BIAS_BF16, out=None)
 
     def forward(self, kind, slot):
         """hit: `hidden_states += residual_cache[slot]` (:221-222) | miss: the 60 blocks, residual into the slot (:224-239); then the

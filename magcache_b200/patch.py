@@ -44,8 +44,8 @@ def _cached_engine(self, attr, build):
 def invalidate_engine(model):
     """Drop the engine cached on `model` (and with it the repacked bf16 copy of the weights, the workspaces and any captured CUDA
     graphs) and its controllers. The engine snapshots the module's parameters at the first forward: call this after anything that
-    changes them — a LoRA merge (on a FLUX model only one whose LoRA layers are then removed before the next forward, see
-    lora.FluxLoraScan), `load_state_dict`, `.to(...)` — and the next forward repacks. The module's own parameters stay
+    changes them — a LoRA merge (on a FLUX or Qwen-Image model only one whose LoRA layers are then removed before the next
+    forward, see lora.LoraScan), `load_state_dict`, `.to(...)` — and the next forward repacks. The module's own parameters stay
     resident next to the packed copy (about +2.8 GB for the 1.3B model, +28 GB for 14B); free or offload them yourself if that matters."""
     for name in ENGINE_ATTRS + ("_mc_ctrls",):
         model.__dict__.pop(name, None)
@@ -584,19 +584,30 @@ def init_magcache_hunyuan(transformer, infer_steps=50, thresh=0.24, K=6, retenti
 # Qwen-Image / Qwen-Image-Edit (MagCache4QwenImage/magcache_generate.py, MagCache4QwenImageEdit/magcache_generate.py: the same
 # forward, calibration and installation statements) on the MMDiT engine
 # ------------------------------------------------------------------------------------------------------------------
-def _qwen_stage(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens, guidance,
-                attention_kwargs):
+def _qwen_lora_scale(self, attention_kwargs):
+    """The call's LoRA scale (magcache_generate.py:185-192: a copy of `attention_kwargs` with "scale" popped; the caller's dict is
+    left as it is). Only the "scale" key is built, and a scale other than 1.0 needs a model with LoRA layers."""
+    extra = dict(attention_kwargs or {})
+    lora_scale = extra.pop("scale", 1.0)
+    if extra:
+        raise NotImplementedError(f"magcache_b200: the Qwen-Image engine takes only the LoRA 'scale' in attention_kwargs; got "
+                                  f"{sorted(extra)}")
+    if lora_scale != 1.0 and not (isinstance(self, torch.nn.Module) and any(is_lora_layer(m) for m in self.modules())):
+        raise NotImplementedError(f"magcache_b200: attention_kwargs scale={lora_scale} but the model has no LoRA layer to scale")
+    return lora_scale
+
+
+def _qwen_stage(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens, guidance):
+    """Stages one Qwen-Image call on the engine (inside `_lora_scaled`) and hands it the adapters as they are now."""
     if guidance is not None:
         raise NotImplementedError("magcache_b200: Qwen-Image guidance (guidance_embeds checkpoints) is not supported")
-    extra = dict(attention_kwargs or {})
-    scale = extra.pop("scale", 1.0)
-    if extra or scale != 1.0:
-        raise NotImplementedError(f"magcache_b200: the Qwen-Image engine takes no attention_kwargs but scale 1.0; got {attention_kwargs}")
     if self.__dict__.get("_mc_shard_kw", {}).get("shard_world", 1) > 1:
         raise NotImplementedError("magcache_b200: the Qwen-Image engine has no token-sharded path; run it on one GPU")
     if not hidden_states.is_cuda:
         raise RuntimeError("magcache_b200: hidden_states must be CUDA tensors (no CPU path)")
     eng = _cached_engine(self, "_mc_qwen_engine", lambda **kw: QwenImageEngine(QwenImageWeights.from_module(self, hidden_states.device)))
+    if isinstance(self, torch.nn.Module):  # (a benchmark's MMDiTHandle sets the engine's LoRA pack itself)
+        eng.sync_lora(self)
     eng.stage_inputs(hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens)
     return eng
 
@@ -607,17 +618,21 @@ def magcache_qwen_image_forward(self, hidden_states, encoder_hidden_states=None,
     signature and state attributes (`cnt, num_steps, magcache_thresh, K, retention_ratio, accumulated_ratio / _err / _steps` as
     per-branch lists, `residual_cache` indexed by `cnt % 2`, `mag_ratios`), `(output,)` or an object with `.sample`. One sample per
     call: the pipelines' true CFG makes a cond and an uncond call per step, each with its own text length and residual slot. A
-    hit runs only img_in, the time embedding, the add and the final layer (mmdit.QwenImageEngine)."""
-    eng = _qwen_stage(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens,
-                      guidance, attention_kwargs)
-    slot = int(self.cnt) % 2
-    skip_forward = _ctrl(self, "qwen-image").decide(self)  # :205-219
-    _take_residual(eng, self.residual_cache[slot], slot)
-    out = eng.forward("hit" if skip_forward else "miss", slot)
-    self.residual_cache[slot] = eng.res[slot].view(1, *eng.res[slot].shape)  # :241
-    self.cnt += 1  # :242-244, the reference's own statements: the wrap rebinds an int on the instance and keeps the accumulators
-    if self.cnt >= self.num_steps:
-        self.cnt = 0
+    hit runs only img_in, the time embedding, the add and the final layer (mmdit.QwenImageEngine). Unmerged PEFT LoRA adapters run
+    as tails of the GEMMs of the Linears they adapt (magcache_b200/lora.py), scaled by `attention_kwargs["scale"]` with the
+    reference's scale / unscale statements (:185-192, :249-250) on every call, hit or miss."""
+    lora_scale = _qwen_lora_scale(self, attention_kwargs)
+    with _lora_scaled(self, lora_scale):
+        eng = _qwen_stage(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens,
+                          guidance)
+        slot = int(self.cnt) % 2
+        skip_forward = _ctrl(self, "qwen-image").decide(self)  # :205-219
+        _take_residual(eng, self.residual_cache[slot], slot)
+        out = eng.forward("hit" if skip_forward else "miss", slot)
+        self.residual_cache[slot] = eng.res[slot].view(1, *eng.res[slot].shape)  # :241
+        self.cnt += 1  # :242-244, the reference's own statements: the wrap rebinds an int on the instance and keeps the accumulators
+        if self.cnt >= self.num_steps:
+            self.cnt = 0
     output = out.view(1, *out.shape)
     return _Sample(output) if return_dict else (output,)
 
@@ -626,26 +641,29 @@ def magcache_qwen_image_calibration(self, hidden_states, encoder_hidden_states=N
                                     img_shapes=None, txt_seq_lens=None, guidance=None, attention_kwargs=None, return_dict=True):
     r"""MagCache4QwenImage/magcache_generate.py:94-171: every call runs the blocks; from `cnt >= 2` on the residual is compared with
     the one of the same CFG branch (`residual_cache[cnt % 2]`) and `norm_ratio / norm_std / cos_dis` get one entry each (rounded to 5
-    places), printed per step in the reference's format. At the wrap the lists are printed and only the counter is reset."""
-    eng = _qwen_stage(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens,
-                      guidance, attention_kwargs)
-    slot = int(self.cnt) % 2
-    _take_residual(eng, self.residual_cache[slot], slot)
-    out, stats = eng.calibrate(slot, compare=self.cnt >= 2)
-    if stats is not None:  # :143-153
-        norm_ratio, norm_std, cos_dis = stats
-        self.norm_ratio.append(round(norm_ratio, 5))
-        self.norm_std.append(round(norm_std, 5))
-        self.cos_dis.append(round(cos_dis, 5))
-        print(f"Step {self.cnt}: norm_ratio={norm_ratio:.5f}, norm_std={norm_std:.5f}, cos_dis={cos_dis:.5f}")
-    self.residual_cache[slot] = eng.res[slot].view(1, *eng.res[slot].shape)  # :155
-    self.cnt += 1
-    if self.cnt >= self.num_steps:  # :158-163
-        self.cnt = 0
-        print("\nCalibration Results:")
-        print("norm_ratio:", self.norm_ratio)
-        print("norm_std:", self.norm_std)
-        print("cos_dis:", self.cos_dis)
+    places), printed per step in the reference's format. At the wrap the lists are printed and only the counter is reset. LoRA
+    adapters and scale as in the forward (:106-113, :168-169)."""
+    lora_scale = _qwen_lora_scale(self, attention_kwargs)
+    with _lora_scaled(self, lora_scale):
+        eng = _qwen_stage(self, hidden_states, encoder_hidden_states, encoder_hidden_states_mask, timestep, img_shapes, txt_seq_lens,
+                          guidance)
+        slot = int(self.cnt) % 2
+        _take_residual(eng, self.residual_cache[slot], slot)
+        out, stats = eng.calibrate(slot, compare=self.cnt >= 2)
+        if stats is not None:  # :143-153
+            norm_ratio, norm_std, cos_dis = stats
+            self.norm_ratio.append(round(norm_ratio, 5))
+            self.norm_std.append(round(norm_std, 5))
+            self.cos_dis.append(round(cos_dis, 5))
+            print(f"Step {self.cnt}: norm_ratio={norm_ratio:.5f}, norm_std={norm_std:.5f}, cos_dis={cos_dis:.5f}")
+        self.residual_cache[slot] = eng.res[slot].view(1, *eng.res[slot].shape)  # :155
+        self.cnt += 1
+        if self.cnt >= self.num_steps:  # :158-163
+            self.cnt = 0
+            print("\nCalibration Results:")
+            print("norm_ratio:", self.norm_ratio)
+            print("norm_std:", self.norm_std)
+            print("cos_dis:", self.cos_dis)
     output = out.view(1, *out.shape)
     return _Sample(output) if return_dict else (output,)
 

@@ -7,6 +7,7 @@ usage (GPU): python tools/bench_mmdit.py flux|hunyuan [--steps N] [--no-cache] [
              python tools/bench_mmdit.py flux --lora RANK [--rounds R] [--steps N]
              python tools/bench_mmdit.py flux --ip-adapter A[,T] [--rounds R] [--steps N]
              python tools/bench_mmdit.py qwen-image [--edit] [--rounds R] [--steps N]
+             python tools/bench_mmdit.py qwen-image [--edit] --lora RANK [--rounds R] [--steps N]
 
 --controlnet D,S: the FLUX 1024^2 miss forward (the whole block stack) with D double-block and S single-block synthetic bf16
 ControlNet samples (S = 0: none for the single blocks) against the same forward without samples, timed in alternating rounds of N
@@ -23,7 +24,12 @@ alternating rounds as for --controlnet; then `mc_ip_attn` alone at 4096 rows wit
 qwen-image: Qwen-Image (60 blocks, 3072 wide, synthetic weights) at 1328^2 (6889 image tokens; --edit: Qwen-Image-Edit's 1024^2
 noised latents plus a 1024^2 reference image, 8192 tokens) with a 200-token cond and a 6-token uncond prompt: cond miss, uncond
 miss and hit medians (CUDA events, alternating rounds of N forwards), peak memory, and the 50-step transformer time of the
-qwen-image-E006K2R02 schedule from those medians."""
+qwen-image-E006K2R02 schedule from those medians.
+
+qwen-image --lora RANK: the cond (200-token) miss and hit forwards with one synthetic rank-RANK adapter on every covered target
+(every block attention and MLP Linear, img_mod.1 / txt_mod.1, img_in, txt_in, norm_out.linear, proj_out; lora.QWEN) against the
+same forwards without adapters, alternating rounds as for --controlnet; then the miss's down-projections alone (one plain GEMM per
+distinct adapted input, N = the padded rank), so the added miss time splits into down-projections and tails."""
 import argparse
 import json
 import os
@@ -250,6 +256,96 @@ def bench_qwen_image(edit, rounds, per_round):
                       "E006K2R02_50_steps_s": total / 1e3, "hits": int(sum(mask)), "calls": len(mask)}))
 
 
+def _qwen_engine(edit):
+    """A Qwen-Image engine on synthetic weights with the cond (200 text tokens) and uncond (6) inputs of one step: (engine, its
+    `_alternate` stand-in, {text tokens: staging function}, image tokens, generator)."""
+    dev = torch.device("cuda:0")
+    g = torch.Generator(device=dev).manual_seed(0)
+    eng = mmdit.QwenImageEngine(mmdit.random_qwen_weights(dev))
+    shapes = [[(1, 64, 64), (1, 64, 64)]] if edit else [(1, 83, 83)]
+    n_img = 8192 if edit else 6889
+    hs = torch.randn(1, n_img, 64, device=dev, generator=g).bfloat16()
+    enc = {n: torch.randn(1, n, 3584, device=dev, generator=g).bfloat16() for n in (200, 6)}
+    t = torch.tensor([0.6], device=dev)
+    slot = {200: 0, 6: 1}
+    stage = {n: (lambda n=n: eng.stage_inputs(hs, enc[n], None, t, shapes, [n])) for n in enc}
+
+    class Slotted:  # `_alternate` calls forward(kind); the slot follows the branch
+        def __init__(self):
+            self.n = 200
+
+        def forward(self, kind):
+            return eng.forward(kind, slot[self.n])
+
+    sl = Slotted()
+    return eng, sl, {n: (lambda n=n, f=f: (setattr(sl, "n", n), f())) for n, f in stage.items()}, n_img, g
+
+
+def bench_qwen_lora(edit, rank, rounds, per_round):
+    """Cond miss and hit forwards at 1328^2 (Edit: 2 x 1024^2) without adapters and with one rank-`rank` adapter (scaling 1) on
+    every covered target, alternating; then the down-projections of one miss alone."""
+    from magcache_b200.lora import QWEN, LoraPack
+    torch.cuda.reset_peak_memory_stats()
+    eng, sl, stage, n_img, g = _qwen_engine(edit)
+    w, dev, D = eng.w, eng.device, eng.w.dim
+    weights = torch.cuda.memory_allocated()
+
+    def ad(n_out, n_in):
+        A = (torch.randn(rank, n_in, device=dev, generator=g) / n_in ** 0.5).bfloat16()
+        return [(A, (0.02 * torch.randn(n_out, rank, device=dev, generator=g)).bfloat16(), 1.0)]
+
+    spec = {}
+    for i in range(len(w.double)):
+        for t, (o, k) in {"attn.to_q": (D, D), "attn.to_k": (D, D), "attn.to_v": (D, D), "attn.to_out.0": (D, D), "attn.add_q_proj": (D, D),
+                          "attn.add_k_proj": (D, D), "attn.add_v_proj": (D, D), "attn.to_add_out": (D, D), "img_mlp.net.0.proj": (4 * D, D),
+                          "img_mlp.net.2": (D, 4 * D), "txt_mlp.net.0.proj": (4 * D, D), "txt_mlp.net.2": (D, 4 * D),
+                          "img_mod.1": (6 * D, D), "txt_mod.1": (6 * D, D)}.items():
+            spec[("double", i, t)] = ad(o, k)
+    for t, (o, k) in {"img_in": (D, w.in_channels), "txt_in": (D, w.joint_dim), "proj_out": (w.out_w.shape[0], D),
+                      "norm_out.linear": (2 * D, D)}.items():
+        spec[("top", 0, t)] = ad(o, k)
+    adapters = torch.cuda.memory_allocated() - weights
+    pack = LoraPack(w, spec, family=QWEN)
+    packed = torch.cuda.memory_allocated() - weights - adapters
+
+    def set_lora(p):
+        stage[200]()
+        eng.lora = p
+
+    stage[6]()  # both workspaces exist, as in a pipeline run
+    times = _alternate(sl, {"plain": lambda: set_lora(None), "lora": lambda: set_lora(pack)}, ("miss", "hit"), rounds, per_round)
+    # the down-projections of one miss alone: every group's input is still staged from the last miss
+    set_lora(pack)
+    sl.forward("miss")
+    groups = list(pack.groups.values()) + [gr for b in pack.double for gr in b["lora"].values()]
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    down = []
+    for _ in range(rounds):
+        torch.cuda.synchronize()
+        e0.record()
+        for _ in range(per_round):
+            for gr in groups:
+                ops.gemm(gr.src, gr.A, out=gr.u)
+        e1.record()
+        torch.cuda.synchronize()
+        down.append(e0.elapsed_time(e1) / per_round)
+    down_bytes = sum(gr.src.shape[0] * gr.src.shape[1] * 2 + gr.A.numel() * 2 + gr.u.numel() * 2 for gr in groups)
+    name, power = card()
+    med = {f"ms_{k}_{kind}": round(statistics.median(v), 3) for (k, kind), v in times.items()}
+    added = med["ms_lora_miss"] - med["ms_plain_miss"]
+    print(json.dumps({"family": "qwen-image-edit" if edit else "qwen-image", "workload": "cond (200-token) forward", "image_tokens": n_img,
+                      "lora_rank": rank, "lora_targets": len(spec), **med, "ms_added_miss": round(added, 3),
+                      "ms_added_hit": round(med["ms_lora_hit"] - med["ms_plain_hit"], 3),
+                      "ms_down_projections_miss": round(statistics.median(down), 3),
+                      "ms_tails_and_rest_miss": round(added - statistics.median(down), 3),
+                      "down_projection_launches": len(groups), "down_projection_GB": round(down_bytes / 1e9, 2),
+                      "spread_ms": {f"{k}_{kind}": [round(min(v), 3), round(max(v), 3)] for (k, kind), v in times.items()},
+                      "spread_down_ms": [round(min(down), 3), round(max(down), 3)],
+                      "adapter_weights_gb": round(adapters / 1e9, 3), "packed_gb": round(packed / 1e9, 3),
+                      "peak_gib": round(torch.cuda.max_memory_allocated() / 2**30, 2),
+                      "rounds": rounds, "forwards_per_round": per_round, "gpu": name, "power_limit": power}))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("family", choices=["flux", "hunyuan", "qwen-image"])
@@ -259,10 +355,13 @@ def main():
     ap.add_argument("--frames", type=int, default=33, help="hunyuan: latent frames (33 = 129 video frames)")
     ap.add_argument("--controlnet", default=None, help="flux: D,S double / single ControlNet samples; times the miss forward with and without")
     ap.add_argument("--controlnet-repeat", action="store_true", help="controlnet_blocks_repeat (XLabs): double block i reads sample i %% D")
-    ap.add_argument("--lora", type=int, default=None, help="flux: rank of one adapter on every covered target; times miss and hit forwards with and without")
+    ap.add_argument("--lora", type=int, default=None, help="flux, qwen-image: rank of one adapter on every covered target; times miss and hit forwards with and without")
     ap.add_argument("--ip-adapter", default=None, help="flux: A[,T] IP-Adapters of T image-prompt tokens (default 16); times miss and hit forwards with and without")
     ap.add_argument("--rounds", type=int, default=5, help="--controlnet / --lora / --ip-adapter: alternating rounds")
     args = ap.parse_args()
+    if args.family == "qwen-image" and args.lora is not None:
+        bench_qwen_lora(args.edit, args.lora, args.rounds, args.steps or 3)
+        return
     if args.family == "qwen-image":
         bench_qwen_image(args.edit, args.rounds, args.steps or 3)
         return
