@@ -361,16 +361,19 @@ class MMDiTCore:
         attention the K|V rows of a rank's image tokens travel through the same exchange as the Wan engine's (`shard.make_exchange`:
         copy-engine pushes into every peer's gathered buffer, consumed segment by segment inside the attention kernel; or the
         all-gather formulation), and the text K|V rows are written locally behind the image rows of the gathered buffer — the key
-        order [image | text] differs from the unsharded engine's, which a softmax over keys cannot see."""
+        order [image | text] differs from the unsharded engine's, which a softmax over keys cannot see. Image token counts that do
+        not divide by the world size follow the pad rule (shard.TokenShard): rank r owns image rows [r ceil(N/P), min((r+1)
+        ceil(N/P), N)), so the last rank carries fewer, and the keys stay [N image rows | text rows] with no pad row among them."""
         D, dev = self.w.dim, self.device
         bf = dict(dtype=torch.bfloat16, device=dev)
         self.n_img_total, self.n_txt = n_img, n_txt
         self.shard = None
         if getattr(self, "world", 1) > 1:
             from .shard import TokenShard
+            # the last rank owns the fewest rows: checking it on every rank makes all of them refuse a count that leaves it none,
+            # instead of one rank raising while the others wait for it in the exchange
+            TokenShard(self.world - 1, self.world, n_img)
             self.shard = TokenShard(self.rank, self.world, n_img, self.group)
-            if self.shard.pad:
-                raise NotImplementedError(f"magcache_b200: {n_img} image tokens over {self.world} ranks needs the pad rule, built for the Wan engines only")
             n_img = self.shard.n_local
         S = n_img + n_txt                      # rows this rank carries
         Sg = self.n_img_total + n_txt          # keys every query attends to
@@ -487,13 +490,19 @@ class MMDiTCore:
         ops.attention(self.qk[:, :D], self.qk[:, D:], self.v, H, out=out, tag="mmdit_attn")
 
     def _gather_output(self, o_local):
-        """Per-token head output of this rank's image rows -> all image rows, replicated (tiny: 64 features per token)."""
+        """Per-token head output of this rank's image rows -> all image rows, replicated (tiny: 64 features per token). The gather
+        moves ceil(N/P) rows per rank: the last rank's pad slots are zero-filled and dropped from the result."""
         if self.shard is None:
             return o_local
         from .shard import gather_rows
-        full = torch.empty(self.n_img_total, o_local.shape[1], dtype=o_local.dtype, device=o_local.device)
-        gather_rows(o_local.contiguous(), full, self.shard.group)
-        return full
+        sh = self.shard
+        loc = o_local.contiguous()
+        if sh.n_local < sh.n_slots:
+            loc = torch.zeros(sh.n_slots, o_local.shape[1], dtype=o_local.dtype, device=o_local.device)
+            loc[:sh.n_local] = o_local
+        full = torch.empty(sh.n_padded, o_local.shape[1], dtype=o_local.dtype, device=o_local.device)
+        gather_rows(loc, full, sh.group)
+        return full[:self.n_img_total]
 
     def run_blocks(self, ctrl=None, ip=None):
         """Double-stream then single-stream blocks (magcache_flux.py:343-424; magcache_sample_video.py:108-139) on `hs`; the image rows of

@@ -55,8 +55,11 @@ def invalidate_engine(model):
 def enable_token_shard(model, rank, world, group=None):
     """Shard the token axis of `model`'s forwards over `world` ranks of one node (call before the first forward; needs an
     initialised torch.distributed NCCL group). Every rank must then make the same calls with the same inputs; outputs are
-    replicated, the residual cache stays sharded. Wan engines shard all tokens; the FLUX / HunyuanVideo engines shard the image tokens and
-    replicate the text tokens. The Open-Sora engine has no token-sharded path: its forward raises NotImplementedError for world > 1
+    replicated, the residual cache stays sharded. Wan engines shard all tokens; the FLUX / Kontext / HunyuanVideo engines shard the
+    image tokens (Kontext: target and reference tokens together) and replicate the text tokens. Any token count N is accepted as long
+    as every rank owns a row (N > (world - 1) * ceil(N / world); otherwise the first forward raises ValueError): rank r owns rows
+    [r * ceil(N / world), min((r + 1) * ceil(N / world), N)), so the last rank carries fewer when N does not divide by the world size
+    (the pad rule of videosys/core/comm.py:373-381). The Qwen-Image engine has no token-sharded path. The Open-Sora engine has no token-sharded path: its forward raises NotImplementedError for world > 1
     (`enable_sequence_parallel` shards it by frames and positions instead)."""
     if any(k in model.__dict__ for k in ENGINE_ATTRS):
         raise RuntimeError("enable_token_shard must be called before the first forward")

@@ -20,6 +20,9 @@ Two exchanges implement the same interface (`KVExchange`):
 Token counts that are not a multiple of the world size follow the reference's pad rule (videosys/core/comm.py:373-381: pad the
 sequence to the next multiple, split equally, drop the pad after the gather): every rank owns ceil(N / P) row SLOTS, the last
 rank's trailing slots are pad — never computed, never attended to (the key count stays N).
+
+An exchange built with `extra_rows` (MMDiT: the replicated text K|V rows every rank writes for itself) gathers the key rows
+[N token rows | extra rows] with no pad slot between them, whatever the pad: the key count is N + extra_rows.
 """
 import ctypes
 import os
@@ -100,11 +103,13 @@ class CollectiveExchange:
     p2p = False
 
     def __init__(self, shard: TokenShard, width, out_shape, device, extra_rows=0):
-        assert extra_rows == 0 or shard.pad == 0, "locally written tail rows follow the token rows directly: no pad slots in between"
         self.sh, self.device, self.out_shape, self.extra = shard, device, tuple(out_shape), extra_rows
         bf = dict(dtype=torch.bfloat16, device=device)
         self.kv_loc = torch.zeros(shard.n_slots, width, **bf)          # pad slots stay zero
         self.kv_all = torch.empty(shard.n_padded + extra_rows, width, **bf)
+        # the all-gather needs equal counts, so its pad slots land in kv_all[N:n_padded]: with a pad, the tail rows are written
+        # apart and copied to kv_all[N:] once the gather has landed (`keys_values`); without one they are written there directly
+        self._tail = torch.empty(extra_rows, width, **bf) if extra_rows and shard.pad else None
         self._work = None
         # MC_SHARD_NCCL=capi (CUDA): the gather is `mc_allgather_kv` — ncclAllGather behind the C ABI on a communicator of this
         # exchange's own (csrc/nccl_gather.cu) — instead of torch.distributed's; same buffers, same ordering
@@ -130,7 +135,7 @@ class CollectiveExchange:
 
     def tail_rows(self, i):
         """The `extra_rows` key rows behind the token rows that every rank writes for itself (MMDiT: the replicated text tokens)."""
-        return self.kv_all[self.sh.n_padded:]
+        return self.kv_all[self.sh.n_padded:] if self._tail is None else self._tail
 
     def begin(self, i):
         if self._nccl is not None:  # on a side stream, so that the q projection overlaps it like the async c10d gather does
@@ -151,6 +156,8 @@ class CollectiveExchange:
             torch.cuda.current_stream().wait_event(self._done)
         else:
             self._work.wait()
+        if self._tail is not None:  # over the gathered pad slots, after the gather that wrote them
+            self.kv_all[self.sh.n_tokens:self.sh.n_tokens + self.extra].copy_(self._tail)
         return self.kv_all[:self.sh.n_tokens + self.extra], {}
 
     def head_output(self, slot):
@@ -189,7 +196,6 @@ class P2PExchange:
         from . import _lib
         self._lib = _lib
         lib, check = _lib.lib, _lib.check
-        assert extra_rows == 0 or shard.pad == 0, "locally written tail rows follow the token rows directly: no pad slots in between"
         self.sh, self.device, self.out_shape, self.width, self.extra = shard, device, tuple(out_shape), width, extra_rows
         P = shard.world
         out_numel = 1
@@ -197,7 +203,8 @@ class P2PExchange:
             out_numel *= v
         self.out_bytes = (out_numel * 4 + 255) // 256 * 256
         self.kv_bytes = ((shard.n_padded + extra_rows) * width * 2 + 255) // 256 * 256
-        self.seg_bytes = shard.n_slots * width * 2
+        # each rank pushes its valid rows only: the last rank's pad slots [N, n_padded) of a peer's buffer hold that peer's tail rows
+        self.seg_bytes = shard.n_local * width * 2
         total = self.FLAG_BYTES + 2 * self.out_bytes + 2 * self.kv_bytes
         ptr = ctypes.c_void_p()
         handle = ctypes.create_string_buffer(64)
@@ -224,8 +231,10 @@ class P2PExchange:
         self.kv = [self.window[k0 + i * self.kv_bytes:k0 + i * self.kv_bytes + (shard.n_padded + extra_rows) * width * 2].view(torch.bfloat16)
                    .view(shard.n_padded + extra_rows, width) for i in range(2)]
         if extra_rows:
-            # the attention kernel waits on the flag of every segment a KV tile touches; the tail rows are local, their
-            # "segments" (indices P ...) are permanently published
+            # the attention kernel waits on the flag of every segment a KV tile touches (segment s = rows [s n_slots, (s+1) n_slots)).
+            # The tail rows [N, N + extra_rows) are local. With a pad, the first of them fall in segment P-1, so a tile there also
+            # waits for the last rank's flag, which every exchange publishes (pushed by that rank, bumped by itself before its own
+            # attention): no tile waits on a flag that never comes. The rest are in segments P ..., permanently published here.
             n_tail = (extra_rows + shard.n_slots - 1) // shard.n_slots + 1
             assert P + n_tail <= 64, "flag table: 64 entries per exchange parity"
             flags[P:P + n_tail] = 0x7FFFFFFF
@@ -249,9 +258,9 @@ class P2PExchange:
 
     def tail_rows(self, i):
         """The `extra_rows` key rows behind the token rows of gathered buffer i, written by every rank for itself (MMDiT: the
-        replicated text tokens); call after `own_rows(i)` (which orders the stream behind the pushes that last read the buffer — they
-        never touch the tail, but the attention that last read it is ordered the same way)."""
-        return self.kv[i][self.sh.n_padded:]
+        replicated text tokens), directly after the N token rows; call after `own_rows(i)` (which orders the stream behind the pushes
+        that last read the buffer — they never touch the tail, but the attention that last read it is ordered the same way)."""
+        return self.kv[i][self.sh.n_tokens:self.sh.n_tokens + self.extra]
 
     def begin(self, i):
         lib, check = self._lib.lib, self._lib.check
