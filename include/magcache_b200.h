@@ -474,6 +474,21 @@ int32_t mc_head_unpatchify_step(const void* x, int32_t x_dtype, const float* r_o
                                 int32_t F, int32_t Hp, int32_t Wp, int32_t C_out, float eps, float* const* outs, int32_t n_out,
                                 const void* prepared, int64_t prepared_bytes, int32_t flags, const float* cond, const float* x_latent,
                                 float guide_scale, float coef_x, float coef_v, void* stream);
+/* mc_head_unpatchify_step with one history term and the x0-prediction: the scheduler update of a multistep solver with one stored
+ * tensor (FlowDPM++ 2M, `sample_solver == 'dpm++'`: MagCache4Wan2.1/magcache_generate.py:728-731, the caller loop
+ * eval/magcache/experiments/Wan2.1_EVAL/wan_magcache.py:301-310). With y the unconditional prediction it stores
+ *     v   = y + guide_scale * (cond - y)
+ *     out = coef_x * x_latent + coef_v * v + coef_h * hist
+ *     x0  = x_latent - sigma * v                      (to x0_out when it is not NULL)
+ * every product and sum rounded separately in that order: bit-equal to mc_head_unpatchify_ex followed by mc_cfg_step with
+ * hist = {hist}, coef_h = {coef_h}, sigma, x0_out. hist and x0_out are fp32 in the output layout [C, F, 2Hp, 2Wp], read / written
+ * at the positions of the launch's tokens only. out may alias x_latent; hist may not alias an output, x0_out may not alias an
+ * output, x_latent or cond. cond, x_latent, hist, x0_out 8-byte aligned. */
+int32_t mc_head_unpatchify_step_hist(const void* x, int32_t x_dtype, const float* r_or_null, int64_t rows, int64_t row_offset, int32_t cols,
+                                     int32_t F, int32_t Hp, int32_t Wp, int32_t C_out, float eps, float* const* outs, int32_t n_out,
+                                     const void* prepared, int64_t prepared_bytes, int32_t flags, const float* cond, const float* x_latent,
+                                     float guide_scale, float coef_x, float coef_v, const float* hist, float coef_h, float sigma,
+                                     float* x0_out, void* stream);
 
 /* Open-Sora 1.2's final layer in one pass (csrc/opensora_head.cu): T2IFinalLayer (videosys/models/transformers/
  * open_sora_transformer_3d.py:50-86) and `unpatchify` (:625-647), replacing OpenSoraEngine.head's mc_ln_modulate (mode 2) per

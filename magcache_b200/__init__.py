@@ -9,7 +9,7 @@ from .config import FAMILIES, PRESETS, MagCacheConfig, interp_cfg, nearest_inter
 from .patch import (enable_sequence_parallel, enable_token_shard, invalidate_engine, init_magcache, init_magcache_calibration, magcache_branch, magcache_calibration,  # noqa: F401
                     init_magcache_eval, init_magcache_flux, init_magcache_flux_calibration, init_magcache_hunyuan, init_magcache_hunyuan_calibration, init_magcache_qwen_image, init_magcache_qwen_image_calibration, init_magcache_wan22, init_teacache, magcache_eval_forward, magcache_flux_calibration, magcache_flux_forward, magcache_forward, magcache_hunyuan_calibration, magcache_hunyuan_forward, magcache_opensora_forward, magcache_qwen_image_calibration, magcache_qwen_image_forward, init_magcache_opensora, magcache_vace_calibration, magcache_vace_forward, magcache_wan22_forward, reset_magcache,
                     teacache_forward, teacache_opensora_forward, init_teacache_opensora)
-from .sampler import FlowEulerSampler, FlowUniPCSampler, cfg_denoise_step, sampling_sigmas  # noqa: F401
+from .sampler import FlowDPMSolverSampler, FlowEulerSampler, FlowUniPCSampler, cfg_denoise_step, sampling_sigmas  # noqa: F401
 from .wan import WAN_CONFIGS, WanDims, WanEngine, WanModelHandle, WanWeights  # noqa: F401
 from .native import NativeWanForward  # noqa: F401
 from .opensora import OpenSoraEngine, OpenSoraWeights, random_opensora_weights  # noqa: F401

@@ -68,6 +68,11 @@ struct HeadParams {
   const float* step_cond;  // nullptr: plain head
   const float* step_x;
   float step_g, step_cx, step_cv;
+  // head_tc_kernel<HIT, true> only (mc_head_unpatchify_step_hist): one history term of a multistep solver, out += coef_h * hist,
+  // and the x0-prediction x - sigma * v stored to step_x0 when it is given (DPM++ 2M keeps it for the next step)
+  const float* step_hist;
+  float* step_x0;
+  float step_ch, step_sigma;
 };
 
 // ---- per-forward preparation: W' = (1 + e1) * W split into bf16 hi / lo, K-major [64, cols]; c1, c0 ----------------------------
@@ -132,7 +137,9 @@ struct HeadMaps {
   CUtensorMap f32_full, f32_tail, bf16_full, bf16_tail, w_hi, w_lo;
 };
 
-template <bool HIT>
+// HIST: the fused step with a history operand and the x0 output (mc_head_unpatchify_step_hist); the HIST = false instantiations are
+// the plain head and mc_head_unpatchify_step, whose code the HIST branches do not touch.
+template <bool HIT, bool HIST = false>
 __global__ void __launch_bounds__(hd::kThreads, 1) head_tc_kernel(const __grid_constant__ HeadMaps maps, const HeadParams p) {
   using namespace hd;
   using L = Layout<HIT>;
@@ -383,16 +390,20 @@ __global__ void __launch_bounds__(hd::kThreads, 1) head_tc_kernel(const __grid_c
         const int H2 = p.Hp * 2, W2 = p.Wp * 2;
         const int64_t plane = static_cast<int64_t>(p.F) * H2 * W2;
         const int64_t off = (static_cast<int64_t>(f) * H2 + hp * 2 + qh) * W2 + wp * 2;
-        const bool step = p.step_cond != nullptr && elive;
+        const bool step = (HIST || p.step_cond != nullptr) && elive;
         // fused caller step: the conditional prediction and the latent at this thread's 16 output positions, fetched in two batches
         // of 8 channels; the first batch is in flight while the last MMAs of the tile finish (x may alias out: every position is
-        // read by the thread that later writes it, before it writes it)
-        float2 cc[8], xl[8];
+        // read by the thread that later writes it, before it writes it). HIST: the history term at the same positions too, in four
+        // batches of 4 channels (three operands per position: the registers of two batches of 8)
+        constexpr int kB = HIST ? 4 : 8;
+        float2 cc[kB], xl[kB];
+        [[maybe_unused]] float2 hl[kB];
         auto fetch = [&](int c0) {
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
+          for (int c = 0; c < kB; ++c) {
             cc[c] = *reinterpret_cast<const float2*>(p.step_cond + (c0 + c) * plane + off);
             xl[c] = *reinterpret_cast<const float2*>(p.step_x + (c0 + c) * plane + off);
+            if constexpr (HIST) hl[c] = *reinterpret_cast<const float2*>(p.step_hist + (c0 + c) * plane + off);
           }
         };
         if (step) fetch(0);
@@ -400,10 +411,10 @@ __global__ void __launch_bounds__(hd::kThreads, 1) head_tc_kernel(const __grid_c
         if (elive) {
           const float2 ms = stats[er];
 #pragma unroll
-          for (int cb = 0; cb < 16; cb += 8) {
+          for (int cb = 0; cb < 16; cb += kB) {
             if (step && cb != 0) fetch(cb);
 #pragma unroll
-            for (int ci = 0; ci < 8; ++ci) {
+            for (int ci = 0; ci < kB; ++ci) {
               const int c = cb + ci;
               const int j0 = qh * 32 + c, j1 = j0 + 16;
               float y0 = fmaf(ms.y, acc[c] - ms.x * __ldg(p.c1 + j0), __ldg(p.c0 + j0));
@@ -414,6 +425,13 @@ __global__ void __launch_bounds__(hd::kThreads, 1) head_tc_kernel(const __grid_c
                 const float v1 = __fadd_rn(y1, __fmul_rn(p.step_g, __fsub_rn(cc[ci].y, y1)));
                 y0 = __fadd_rn(__fmul_rn(p.step_cx, xl[ci].x), __fmul_rn(p.step_cv, v0));
                 y1 = __fadd_rn(__fmul_rn(p.step_cx, xl[ci].y), __fmul_rn(p.step_cv, v1));
+                if constexpr (HIST) {  // cfg_step_one with one history term: + coef_h * h, then x0 = x - sigma * v
+                  y0 = __fadd_rn(y0, __fmul_rn(p.step_ch, hl[ci].x));
+                  y1 = __fadd_rn(y1, __fmul_rn(p.step_ch, hl[ci].y));
+                  if (p.step_x0)
+                    *reinterpret_cast<float2*>(p.step_x0 + c * plane + off) =
+                        make_float2(__fsub_rn(xl[ci].x, __fmul_rn(p.step_sigma, v0)), __fsub_rn(xl[ci].y, __fmul_rn(p.step_sigma, v1)));
+                }
               }
               for (int o = 0; o < p.n_out; ++o) *reinterpret_cast<float2*>(p.out[o] + c * plane + off) = make_float2(y0, y1);
             }
@@ -472,7 +490,7 @@ int32_t mc_head_prepare(const float* head_mod, const float* e, const float* Wt, 
 static int32_t head_launch(const void* x, int32_t x_dtype, const float* r_or_null, int64_t rows, int64_t row_offset, int32_t cols, int32_t F,
                            int32_t Hp, int32_t Wp, int32_t C_out, float eps, float* const* outs, int32_t n_out, const void* prepared,
                            int64_t prepared_bytes, int32_t flags, const float* step_cond, const float* step_x, float step_g, float step_cx,
-                           float step_cv, void* stream) {
+                           float step_cv, const float* step_hist, float step_ch, float step_sigma, float* step_x0, void* stream) {
   using namespace mc;
   MC_CHECK_ARG(x && outs && prepared, "mc_head_unpatchify: null pointer");
   MC_CHECK_ARG(n_out >= 1 && n_out <= hd::kMaxPeers, "mc_head_unpatchify: n_out=%d outside [1, %d]", n_out, hd::kMaxPeers);
@@ -506,6 +524,7 @@ static int32_t head_launch(const void* x, int32_t x_dtype, const float* r_or_nul
   }
   p.n_out = n_out;
   p.step_cond = step_cond, p.step_x = step_x, p.step_g = step_g, p.step_cx = step_cx, p.step_cv = step_cv;
+  p.step_hist = step_hist, p.step_x0 = step_x0, p.step_ch = step_ch, p.step_sigma = step_sigma;
 
   HeadMaps maps{};
   rc = make_tmap_bf16_2d(&maps.w_hi, w_hi, 64, static_cast<uint64_t>(cols), static_cast<uint64_t>(cols), hd::kOut, hd::kKC);
@@ -525,8 +544,16 @@ static int32_t head_launch(const void* x, int32_t x_dtype, const float* r_or_nul
     if (rc) return rc;
   }
   const int grid = static_cast<int>((rows + p.rows_per_cta - 1) / p.rows_per_cta);
-  static PerDeviceOnce once_hit, once_stream;
-  if (r_or_null) {
+  static PerDeviceOnce once_hit, once_stream, once_hist_hit, once_hist_stream;
+  if (step_hist && r_or_null) {
+    rc = set_max_smem_once(head_tc_kernel<true, true>, hd::Layout<true>::kSmem, once_hist_hit, "cudaFuncSetAttribute(head smem)");
+    if (rc) return rc;
+    head_tc_kernel<true, true><<<grid, hd::kThreads, hd::Layout<true>::kSmem, s>>>(maps, p);
+  } else if (step_hist) {
+    rc = set_max_smem_once(head_tc_kernel<false, true>, hd::Layout<false>::kSmem, once_hist_stream, "cudaFuncSetAttribute(head smem)");
+    if (rc) return rc;
+    head_tc_kernel<false, true><<<grid, hd::kThreads, hd::Layout<false>::kSmem, s>>>(maps, p);
+  } else if (r_or_null) {
     rc = set_max_smem_once(head_tc_kernel<true>, hd::Layout<true>::kSmem, once_hit, "cudaFuncSetAttribute(head smem)");
     if (rc) return rc;
     head_tc_kernel<true><<<grid, hd::kThreads, hd::Layout<true>::kSmem, s>>>(maps, p);
@@ -543,7 +570,7 @@ int32_t mc_head_unpatchify_ex(const void* x, int32_t x_dtype, const float* r_or_
                               int32_t F, int32_t Hp, int32_t Wp, int32_t C_out, float eps, float* const* outs, int32_t n_out,
                               const void* prepared, int64_t prepared_bytes, int32_t flags, void* stream) {
   return head_launch(x, x_dtype, r_or_null, rows, row_offset, cols, F, Hp, Wp, C_out, eps, outs, n_out, prepared, prepared_bytes, flags, nullptr,
-                     nullptr, 0.f, 0.f, 0.f, stream);
+                     nullptr, 0.f, 0.f, 0.f, nullptr, 0.f, 0.f, nullptr, stream);
 }
 
 int32_t mc_head_unpatchify_step(const void* x, int32_t x_dtype, const float* r_or_null, int64_t rows, int64_t row_offset, int32_t cols,
@@ -554,7 +581,30 @@ int32_t mc_head_unpatchify_step(const void* x, int32_t x_dtype, const float* r_o
   MC_CHECK_ARG((reinterpret_cast<uintptr_t>(cond) & 7u) == 0 && (reinterpret_cast<uintptr_t>(x_latent) & 7u) == 0,
                "mc_head_unpatchify_step: cond / latent must be 8-byte aligned");
   return head_launch(x, x_dtype, r_or_null, rows, row_offset, cols, F, Hp, Wp, C_out, eps, outs, n_out, prepared, prepared_bytes, flags, cond,
-                     x_latent, guide_scale, coef_x, coef_v, stream);
+                     x_latent, guide_scale, coef_x, coef_v, nullptr, 0.f, 0.f, nullptr, stream);
+}
+
+int32_t mc_head_unpatchify_step_hist(const void* x, int32_t x_dtype, const float* r_or_null, int64_t rows, int64_t row_offset, int32_t cols,
+                                     int32_t F, int32_t Hp, int32_t Wp, int32_t C_out, float eps, float* const* outs, int32_t n_out,
+                                     const void* prepared, int64_t prepared_bytes, int32_t flags, const float* cond, const float* x_latent,
+                                     float guide_scale, float coef_x, float coef_v, const float* hist, float coef_h, float sigma,
+                                     float* x0_out, void* stream) {
+  auto al8 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 7u) == 0; };
+  MC_CHECK_ARG(cond != nullptr && x_latent != nullptr && hist != nullptr, "mc_head_unpatchify_step_hist: null cond / latent / hist");
+  MC_CHECK_ARG(al8(cond) && al8(x_latent) && al8(hist) && (x0_out == nullptr || al8(x0_out)),
+               "mc_head_unpatchify_step_hist: cond / latent / hist / x0_out must be 8-byte aligned");
+  MC_CHECK_ARG(outs != nullptr && n_out >= 1 && n_out <= mc::hd::kMaxPeers, "mc_head_unpatchify_step_hist: outs null or n_out=%d outside [1, %d]",
+               n_out, mc::hd::kMaxPeers);
+  MC_CHECK_ARG(hist != x0_out, "mc_head_unpatchify_step_hist: hist aliases x0_out");
+  MC_CHECK_ARG(x0_out == nullptr || (x0_out != x_latent && x0_out != cond),
+               "mc_head_unpatchify_step_hist: x0_out may not alias the latent or cond (out may alias the latent)");
+  for (int i = 0; i < n_out; ++i) {
+    MC_CHECK_ARG(outs[i] != hist, "mc_head_unpatchify_step_hist: hist aliases out[%d]", i);
+    MC_CHECK_ARG(outs[i] != cond, "mc_head_unpatchify_step_hist: cond aliases out[%d]", i);
+    MC_CHECK_ARG(x0_out == nullptr || outs[i] != x0_out, "mc_head_unpatchify_step_hist: x0_out aliases out[%d]", i);
+  }
+  return head_launch(x, x_dtype, r_or_null, rows, row_offset, cols, F, Hp, Wp, C_out, eps, outs, n_out, prepared, prepared_bytes, flags, cond,
+                     x_latent, guide_scale, coef_x, coef_v, hist, coef_h, sigma, x0_out, stream);
 }
 
 int32_t mc_head_unpatchify(const void* x, int32_t x_dtype, const float* r_or_null, int64_t rows, int64_t row_offset, int32_t cols,

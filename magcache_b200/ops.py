@@ -643,7 +643,7 @@ def head_prepare(head_mod, e, w_t, b, tag=None, slot=0):
 
 
 def head_unpatchify(x, head_mod, e, w_t, b, grid, c_out=16, residual=None, eps=1e-6, tag=None, row_offset=0, out=None, round_sum_to_bf16=False,
-                    peer_outs=None, prep=None, step=None):
+                    peer_outs=None, prep=None, step=None, step_hist=None):
     """head(x, e) + unpatchify (MagCache4Wan2.1/magcache_generate.py:304-305) -> fp32 [c_out, F, 2*Hp, 2*Wp].
     x fp32 (the residual stream), or bf16 with `residual` (fp32): the cache-hit sum x + residual is formed on the fly (fused hit
     path, :295). `prep`: a `head_prepare` result for this forward's time embedding (else it is computed here). A token-sharded
@@ -651,7 +651,10 @@ def head_unpatchify(x, head_mod, e, w_t, b, grid, c_out=16, residual=None, eps=1
     `peer_outs` (device pointers of the peers' outputs) makes the kernel store its rows there as well.
     `step` = (cond, x_latent, guide_scale, coef_x, coef_v): this is the unconditional head of a denoising step and the caller loop's
     CFG combine + scheduler update are applied in the epilogue (`mc_head_unpatchify_step`, SURVEY §8f-1): the result is
-    `coef_x * x_latent + coef_v * (y + guide_scale * (cond - y))` instead of y — bit-equal to this head followed by `cfg_step`."""
+    `coef_x * x_latent + coef_v * (y + guide_scale * (cond - y))` instead of y — bit-equal to this head followed by `cfg_step`.
+    `step_hist` = (hist, coef_h, sigma, x0_out), with `step`: a multistep solver's one history term is added (`+ coef_h * hist`) and
+    the x0-prediction `x_latent - sigma * v` is written into `x0_out` (None: not written) — `mc_head_unpatchify_step_hist`,
+    bit-equal to this head followed by `cfg_step(..., hist=[hist], coef_h=[coef_h], sigma=sigma, x0_out=x0_out)`."""
     import ctypes
     _dev(x)
     F, Hp, Wp = grid
@@ -670,10 +673,20 @@ def head_unpatchify(x, head_mod, e, w_t, b, grid, c_out=16, residual=None, eps=1
     ptrs = [out.data_ptr()] + [int(p) for p in (peer_outs or [])]
     arr = (ctypes.c_void_p * len(ptrs))(*ptrs)
     rptr = residual.data_ptr() if residual is not None else None
+    assert step_hist is None or step is not None, "step_hist extends a fused step"
     with _Timed(tag, "head"):
         if step is None:
             check(lib.mc_head_unpatchify_ex(x.data_ptr(), _dt(x), rptr, rows, row_offset, cols, F, Hp, Wp, c_out, eps, arr, len(ptrs), prep.ptr,
                                             prep.nbytes, 1 if round_sum_to_bf16 else 0, _stream()))
+        elif step_hist is not None:
+            cond, x_lat, g, cx, cv = step
+            hist, ch, sig, x0_out = step_hist
+            for t_ in (cond, x_lat, hist) + ((x0_out,) if x0_out is not None else ()):
+                assert t_.dtype == torch.float32 and t_.is_contiguous() and t_.numel() == out.numel() and t_.device == x.device
+            check(lib.mc_head_unpatchify_step_hist(x.data_ptr(), _dt(x), rptr, rows, row_offset, cols, F, Hp, Wp, c_out, eps, arr, len(ptrs),
+                                                   prep.ptr, prep.nbytes, 1 if round_sum_to_bf16 else 0, cond.data_ptr(), x_lat.data_ptr(),
+                                                   float(g), float(cx), float(cv), hist.data_ptr(), float(ch), float(sig),
+                                                   x0_out.data_ptr() if x0_out is not None else None, _stream()))
         else:
             cond, x_lat, g, cx, cv = step
             for t_ in (cond, x_lat):

@@ -27,14 +27,18 @@ def sampling_sigmas(steps, shift):
     return out
 
 
-def cfg_denoise_step(model, x, t, context, context_null, seq_len, guide_scale, coef_v, coef_x=1.0, forward=None, **kw):
+def cfg_denoise_step(model, x, t, context, context_null, seq_len, guide_scale, coef_v, coef_x=1.0, forward=None, hist=None, coef_h=0.0,
+                     sigma=0.0, x0_out=None, **kw):
     """`x <- coef_x * x + coef_v * (uncond + g * (cond - uncond))` with both predictions from the patched forward of `model`
     (SURVEY §8f rank 1 as written). On the unsharded Wan engine the combine and the update ride in the epilogue of the unconditional
     call's head kernel (`mc_head_unpatchify_step`): the unconditional prediction is never written, no separate pass over the
     latents runs — on a step where both calls hit the cache the whole step is two streaming head launches. Token-sharded engines
     (whose head stores go to every peer) and multistep solvers that keep history terms use `ops.cfg_step` after the two calls.
     Bit-equal either way. `forward(x, t, context) -> prediction` replaces the plain `model([x], t=..., context=[...])` call (a
-    caller that wraps its forwards, e.g. with timing events)."""
+    caller that wraps its forwards, e.g. with timing events).
+    `hist` (one stored tensor of a multistep solver, DPM++ 2M's previous x0-prediction) adds `coef_h * hist` to the update and,
+    with `x0_out`, writes the x0-prediction `x - sigma * v` there: in the same head epilogue (`mc_head_unpatchify_step_hist`) on
+    the fused path, as `ops.cfg_step(..., hist=[hist], ...)` on the others."""
     from .patch import _engine
     if forward is None:
         def forward(xx, tt, cc):
@@ -42,11 +46,18 @@ def cfg_denoise_step(model, x, t, context, context_null, seq_len, guide_scale, c
     cond = forward(x, t, context)
     eng = _engine(model)
     # the fused form is built for one timestep per call and 16 output channels (not Wan2.2 TI2V-5B: per-token t, 48 channels)
+    if hist is None and x0_out is not None:
+        raise ValueError("magcache_b200: cfg_denoise_step writes x0_out only together with a history term (hist)")
     if getattr(eng, "shard", None) is None and hasattr(eng, "arm_step") and t.numel() == 1 and len(getattr(eng, "head_groups", (0,))) == 1:
-        eng.arm_step(cond, x, guide_scale, coef_x, coef_v, out=x)
+        if hist is None:
+            eng.arm_step(cond, x, guide_scale, coef_x, coef_v, out=x)
+        else:
+            eng.arm_step(cond, x, guide_scale, coef_x, coef_v, out=x, hist=hist, coef_h=coef_h, sigma=sigma, x0_out=x0_out)
         return forward(x, t, context_null)
     uncond = forward(x, t, context_null)
-    return ops.cfg_step(cond, uncond, guide_scale, x, coef_v, coef_x=coef_x, out=x)
+    if hist is None:
+        return ops.cfg_step(cond, uncond, guide_scale, x, coef_v, coef_x=coef_x, out=x)
+    return ops.cfg_step(cond, uncond, guide_scale, x, coef_v, coef_x=coef_x, hist=[hist], coef_h=[coef_h], sigma=sigma, out=x, x0_out=x0_out)
 
 
 class FlowEulerSampler:
@@ -268,4 +279,97 @@ class FlowUniPCSampler:
         if self.lower_order_nums < self.order:
             self.lower_order_nums += 1
         self.i += 1
+        return out
+
+
+class FlowDPMSolverSampler:
+    """DPM-Solver++ (Lu et al. 2022, "DPM-Solver++: Fast Solver for Guided Sampling of Diffusion Probabilistic Models"): data
+    (x0) prediction, multistep, order 2 with the midpoint update, first order on the first step (no history yet) and on the last
+    (lower_order_final: sigma_next = 0), on the flow parameterisation alpha = 1 - sigma, lambda = log(alpha) - log(sigma). It
+    stands in for upstream Wan's `FlowDPMSolverMultistepScheduler` (`--sample_solver dpm++`, MagCache4Wan2.1/magcache_generate.py:
+    728-731, MagCache4Wan2.2/magcache_generate.py:526-529). PARITY UNPINNED: that scheduler is upstream Wan code which is not in the
+    reference tree; what follows restates the published algorithm with the configuration Wan constructs it with, as far as it is
+    known without that source (algorithm "dpmsolver++", solver_order 2, "midpoint", lower_order_final, final sigma 0, the
+    scheduler's own shift 1 over the caller's `sampling_sigmas(steps, shift)`, timestep = 1000 * sigma); none of it could be checked
+    against upstream's code.
+
+    Per step, with s the current and t the next sigma, h = lambda_t - lambda_s, m0 = x - sigma_s * v (v the guided flow
+    prediction) and m1 the previous step's m0:
+        order 1:  x_t = (sigma_t / sigma_s) x - alpha_t (e^-h - 1) m0
+        order 2:  x_t = (sigma_t / sigma_s) x - alpha_t (e^-h - 1) D0 - 1/2 alpha_t (e^-h - 1) D1,   D0 = m0, D1 = (m0 - m1) / r0,
+                  r0 = (lambda_s - lambda_{s-1}) / h
+    folded on the host into float64 scalars, out = cx * x + cv * v + ch * m1 (`coeffs`), and ONE `mc_cfg_step` launch per step that
+    also writes m0 for the next step. The first-order update equals the Euler step x + (sigma_t - sigma_s) v in exact arithmetic
+    (alpha_t (e^-h - 1) = sigma_t / sigma_s - 1). `denoise` folds the launch into the unconditional call's head on the unsharded Wan
+    engine (`cfg_denoise_step` -> `mc_head_unpatchify_step_hist`), so a step whose two calls hit the cache is two head launches.
+    The latent is updated in place; the two x0-prediction buffers are the sampler's own and are recycled."""
+
+    def __init__(self, sigmas, order=2):
+        if order not in (1, 2):
+            raise NotImplementedError("FlowDPMSolverSampler: solver order 1 or 2 (Wan constructs the scheduler with order 2)")
+        self.sigmas = [float(s) for s in sigmas]
+        self.order = order
+        self.i = 0
+        self._m = None  # [previous x0-prediction (zeros before the first step), this step's], device tensors swapped every step
+
+    @property
+    def timestep(self):
+        return 1000.0 * self.sigmas[self.i]
+
+    @staticmethod
+    def _lam(sigma):
+        """lambda = log(1 - sigma) - log(sigma), with the two ends of a flow schedule stated: the terminal sigma 0 has lambda = +inf
+        (its update returns the x0-prediction), sigma 1 (where `sampling_sigmas` starts) has lambda = -inf (h = +inf: e^-h = 0)."""
+        if sigma == 0.0:
+            return math.inf
+        if sigma == 1.0:
+            return -math.inf
+        return math.log(1.0 - sigma) - math.log(sigma)
+
+    def step_order(self, i=None):
+        """1 on the first and the last step, else the solver order."""
+        i = self.i if i is None else i
+        return 1 if self.order == 1 or i == 0 or i == len(self.sigmas) - 2 else 2
+
+    def coeffs(self, i=None):
+        """(cx, cv, ch) of step i, float64: out = cx * x + cv * v + ch * m1."""
+        i = self.i if i is None else i
+        s_s, s_t = self.sigmas[i], self.sigmas[i + 1]
+        h = self._lam(s_t) - self._lam(s_s)
+        a = (1.0 - s_t) * math.expm1(-h)  # alpha_t (e^-h - 1): -alpha_t from sigma_s = 1, -1 into sigma_t = 0
+        ratio = s_t / s_s
+        if self.step_order(i) == 1:
+            # x_t = ratio x - a (x - sigma_s v)
+            return ratio - a, a * s_s, 0.0
+        r0 = (self._lam(s_s) - self._lam(self.sigmas[i - 1])) / h
+        ch = 0.5 * a / r0  # -1/2 a D1 = -(a / (2 r0)) m0 + (a / (2 r0)) m1; 0 after a sigma-1 step (r0 = +inf)
+        b = a + ch         # the whole weight of m0 = x - sigma_s v
+        return ratio - b, b * s_s, ch
+
+    def _bufs(self, like):
+        m = self._m
+        if m is None or m[0].shape != like.shape or m[0].device != like.device or m[0].dtype != like.dtype:
+            m = self._m = [torch.zeros_like(like), torch.zeros_like(like)]
+        return m
+
+    def _advance(self):
+        self._m.reverse()  # this step's x0-prediction is the next step's history
+        self.i += 1
+
+    def step(self, cond, uncond, guide_scale, x):
+        """cond / uncond: the two forwards' outputs at (x, sigma_i), fp32, same shape as x. x is updated in place and returned."""
+        cx, cv, ch = self.coeffs()
+        m1, m0 = self._bufs(x)
+        ops.cfg_step(cond, uncond, guide_scale, x, cv, coef_x=cx, hist=[m1], coef_h=[ch], sigma=self.sigmas[self.i], out=x, x0_out=m0)
+        self._advance()
+        return x
+
+    def denoise(self, model, x, t, context, context_null, seq_len, guide_scale, **kw):
+        """One whole step of the caller loop (wan_magcache.py:296-310), as `FlowEulerSampler.denoise`: cond call, uncond call, CFG
+        combine, scheduler update; the latent `x` [C, F, H, W] is updated in place and returned."""
+        cx, cv, ch = self.coeffs()
+        m1, m0 = self._bufs(x)
+        out = cfg_denoise_step(model, x, t, context, context_null, seq_len, guide_scale, coef_v=cv, coef_x=cx, hist=m1, coef_h=ch,
+                               sigma=self.sigmas[self.i], x0_out=m0, **kw)
+        self._advance()
         return out

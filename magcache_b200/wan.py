@@ -268,7 +268,7 @@ class WanEngine:
         self._nat, self._nat_grid = None, None
         self._slot = 0   # CFG slot of the forward in flight (selects the output window of a sharded engine)
         self.hit_sum_bf16 = False  # TeaCache comparator: the hit sum is rounded to bf16 before the head (wan_teacache.py:569/577)
-        self._step = None          # (cond, x_latent, guide_scale, coef_x, coef_v, out) armed by `arm_step` for the next forward
+        self._step = None          # (cond, x_latent, guide_scale, coef_x, coef_v, out, hist) armed by `arm_step` for the next forward
         # per-token timesteps (Wan2.2, MagCache4Wan2.2/magcache_generate.py:263-272): the distinct values of this call and the
         # contiguous LOCAL row ranges that carry them, [(row0, row1, value index)]; None = one timestep for every token
         self.t_values, self.runs, self._runs_key = 1, None, None
@@ -507,16 +507,21 @@ class WanEngine:
         ops._count(self._nat.launches(skip))
         return out
 
-    def arm_step(self, cond, x_latent, guide_scale, coef_x, coef_v, out=None):
+    def arm_step(self, cond, x_latent, guide_scale, coef_x, coef_v, out=None, hist=None, coef_h=0.0, sigma=0.0, x0_out=None):
         """Fold the caller loop's CFG combine + scheduler update (eval/.../wan_magcache.py:301-310) into the head pass of the NEXT
         forward, which must be the unconditional call of the step whose conditional prediction is `cond`: that forward then returns
         `coef_x * x_latent + coef_v * (uncond + guide_scale * (cond - uncond))` (written into `out`, which may be `x_latent` itself)
-        instead of the unconditional prediction. One-shot; bit-equal to the plain forward followed by `ops.cfg_step`."""
+        instead of the unconditional prediction. One-shot; bit-equal to the plain forward followed by `ops.cfg_step`.
+        `hist` (a multistep solver's one stored tensor, same layout as the latent): `coef_h * hist` is added as well and, with
+        `x0_out`, the x0-prediction `x_latent - sigma * v` is written there (`mc_head_unpatchify_step_hist`; DPM++ 2M)."""
         if self.shard is not None:
             raise NotImplementedError("magcache_b200: the fused step is built for the unsharded engine (sharded runs use ops.cfg_step)")
         if len(self.head_groups) != 1:
             raise NotImplementedError("magcache_b200: the fused step is built for 16 output channels (use ops.cfg_step)")
-        self._step = (cond, x_latent, float(guide_scale), float(coef_x), float(coef_v), out)
+        if hist is None and x0_out is not None:
+            raise ValueError("magcache_b200: arm_step writes x0_out only together with a history term (hist)")
+        h = None if hist is None else (hist, float(coef_h), float(sigma), x0_out)
+        self._step = (cond, x_latent, float(guide_scale), float(coef_x), float(coef_v), out, h)
 
     def forward(self, kind, slot):
         """Run (or replay) one forward of the given kind for CFG slot `slot`; returns a fresh fp32 [C, F, H, W] tensor."""
@@ -712,6 +717,8 @@ class WanEngine:
             (wt, hb), = self.head_groups
             if self.shard is None and self._step is not None:
                 kw["step"], out = self._step[:5], self._step[5]
+                if self._step[6] is not None:
+                    kw["step_hist"] = self._step[6]
             out = ops.head_unpatchify(x, w.head_mod, e, wt, hb, grid, residual=residual, row_offset=row_offset, out=out, peer_outs=peer_outs,
                                       prep=self._head_prep[(0, 0)], **kw)
         else:
